@@ -1,17 +1,22 @@
 #!/usr/bin/env python
-"""bench.py -- tokens/sec of one Llama-3-8B training step under a Galvatron per-layer hybrid strategy on N B200s.
+"""bench.py -- tokens/sec of one Llama-3 training step under a Galvatron per-layer hybrid strategy on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]                      (N > 1: launched under torchrun)
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]  (N > 1: launched under torchrun)
     python bench.py --impl reference [--gpus N] [--steps K] [--warmup W]     (CPU restatement of the reference path)
 
 One "step" = forward_backward over the global batch (chunks microbatches) + optimizer step, through the public API
 (``llama_model_hp`` -> ``GalvatronModel.forward_backward``), on synthetic tokens of the reference's generator
-(``DataLoaderForLlama``) and random-init weights.  Workload at every N: the strategy JSON ``configs/galvatron_config_
-llama3-8b_<N>gpus.json`` (per-GPU batch fixed => weak scaling).  Prints ONE JSON line on rank 0.
+(``DataLoaderForLlama``) and random-init weights.  Workload: the strategy JSON ``configs/galvatron_config_<model>_<N>gpus.json``
+(per-GPU batch fixed => weak scaling): plain ZeRO-2 data parallelism, 8 sequences per GPU in microbatches of one.  The model has
+Llama-3.2-1B shapes (1.50 B parameters, untied embeddings), the Llama-3 size whose training state fits one 80 GB H100: per GPU
+4 B/parameter of bf16 weights + gradients in the arena (6.0 GB) + 12 B/parameter of fp32 master and Adam state sharded over N
+(18.0 GB / N) + the activations of one seq-8192 microbatch (~11 GB with the logits) = 35 GB at N = 1 and less at N > 1.
+Llama-3-8B does not fit: 16 B/parameter is 128 GB before activations on one GPU, and ZeRO-2 at N = 2 still needs 64 + 48 GB.
+Prints ONE JSON line on rank 0.
 
   value      tokens/s with the step's tokens already resident in HBM (CUDA-event timed, max over ranks)
   e2e        the same loop with the tokens/labels copied from pinned host memory every step and the loss read back
-  roofline   the dominant kernel (the tcgen05 GEMM): algorithmic FLOPs / CUDA-event launch time vs the measured cuBLAS peak
+  roofline   the dominant kernel (the wgmma GEMM): algorithmic FLOPs / CUDA-event launch time vs the bf16 peak
   cpu_baseline  the oracle CPU restatement (oracle/gloo_backend.py) on a bounded sample, rank 0 at N=1 only
   probe      two steps on a FIXED batch that is the same on every rank and at every N (loss at init, loss after one update:
              both are N-invariant, so a broken forward or update shows when the driver's N = 1/2/4/8 lines are compared) and,
@@ -20,9 +25,11 @@ llama3-8b_<N>gpus.json`` (per-GPU batch fixed => weak scaling).  Prints ONE JSON
   path_legs  (N >= 2) the collectives north_star names, each as a short fixed-strategy run of the SAME model in a child process
              per rank (a failing leg cannot take the headline down): TP=N Megatron-SP (fused all-gather+GEMM / GEMM+reduce-
              scatter), TP=N (fused GEMM+all-reduce, NVLS), Ulysses SP=N (all-to-all), PP=2 x TP=N/2 1F1B (peer-copy p2p),
-             ZeRO-3 + checkpointing (and Llama-3-70B ZeRO-3 at N=8, BASELINE config 5): tokens/s, per-collective achieved bus
-             GB/s against 900 nominal / 770 measured, and a parity check of the same strategy on the tiny model against the
+             ZeRO-3 + checkpointing (and a 13B ZeRO-3 run at N=8 in place of BASELINE config 5): tokens/s, per-collective achieved bus
+             GB/s against the 450 GB/s nominal NVLink rate, and a parity check of the same strategy on the tiny model against the
              oracle (tests/_host_worker.py: loss 5e-3, per-parameter gradients 3e-2 rel-L2).
+  --dump-outputs DIR  after the timed steps, what the last timed step computed: its loss and a fixed, seeded sample of the updated
+             fp32 master weights of every unit, as DIR/<name>.npy (inputs are seeded, so two builds can be compared output for output)
 """
 import argparse
 import json
@@ -36,8 +43,8 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-METRIC = "tokens/sec Llama-3-8B auto-searched hybrid strategy at 1/2/4/8 B200 vs ref CPU"
-MODEL = "llama3-8b"
+METRIC = "tokens/sec Llama-3.2-1B-shaped ZeRO-2 training step at 1/2/4/8 H100 vs ref CPU"
+MODEL = "llama3.2-1b"
 SEQ = 8192
 PER_GPU_BATCH = 8
 
@@ -66,17 +73,19 @@ def parse():
     p.add_argument("--total-budget-s", type=float, default=760.0, help="wall-clock budget of the whole bench.py run (legs are skipped beyond it)")
     p.add_argument("--no-probe", action="store_true")
     p.add_argument("--legs-only", action="store_true", help="debug: skip the headline run, run the path legs only (prints {\"path_legs\": ...})")
+    p.add_argument("--dump-outputs", default="", metavar="DIR", help="write the last timed step's loss and a seeded sample of the "
+                   "updated weights to DIR/<name>.npy (<= 64 MB)")
     return p.parse_args()
 
 
-def strategy_for(n_gpus, path=None):
-    path = path or os.path.join(ROOT, "configs", "galvatron_config_llama3-8b_%dgpus.json" % n_gpus)
+def strategy_for(n_gpus, model, path=None):
+    path = path or os.path.join(ROOT, "configs", "galvatron_config_%s_%dgpus.json" % (model, n_gpus))
     with open(path) as f:
         return path, json.load(f)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (a power-capped card lowers its clocks under load)."""
 
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -122,24 +131,7 @@ def measured_peaks():
         with open(path) as f:
             d = json.load(f)
         return d.get("bf16_tflops_sustained", d.get("bf16_tflops")), "MEASURED_PEAKS.json bf16_tflops_sustained (measured)"
-    return 1400.0, "B200_PROFILING.md fallback (sustained ~1.4 PFLOP/s)"
-
-
-def ncu_gemm_traffic(flops_per_launch_avg):
-    """DRAM bytes per (average) GEMM launch from the committed `ncu --set full` capture: the capture holds three launches of
-    known shape; their bytes-per-FLOP ratio is applied to the average launch of the timed region."""
-    path = os.path.join(ROOT, "profiles", "r01_ncu_gemm_full_summary.json")
-    try:
-        with open(path) as f:
-            launches = json.load(f)["launches"]
-        to_bytes = lambda s: float(s.split()[0]) * {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}[s.split()[1]]  # noqa: E731
-        total = sum(to_bytes(l["dram__bytes_read.sum"]) + to_bytes(l["dram__bytes_write.sum"]) for l in launches)
-        # the three captured launches: gate/up dgrad [8192x28672]x[28672x4096], o-proj wgrad and dgrad [8192|4096 x 4096 x 4096|8192]
-        flops = 2.0 * 8192 * 4096 * (28672 + 4096 + 4096)
-        return round(total / flops * flops_per_launch_avg), ("dram__bytes_read+write of 3 captured launches (profiles/r01_ncu_gemm_full_summary.json) "
-                                                            "scaled by FLOPs to the average launch of this run")
-    except Exception:  # noqa: BLE001
-        return None, "no ncu capture found"
+    return 989.0, "H100 SXM data sheet, dense BF16 at up to 700 W (not reached; a lower power limit lowers it)"
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -226,7 +218,7 @@ def bert_batch(tokens, labels, vocab_size):
     return tokens, mlm, mask, token_type
 
 
-NVLINK_NOMINAL_GBS, NVLINK_MEASURED_GBS = 900.0, 770.0    # per direction per GPU; measured = peer copy (B200_PROFILING.md)
+NVLINK_NOMINAL_GBS = 450.0    # H100 SXM NVLink 4, per direction per GPU (data sheet)
 T_START = time.time()
 
 
@@ -280,11 +272,11 @@ def reduction_checksum(model, step_fn, world):
 
 
 def summarize_comm(prof, steps):
-    """{kind: calls/step, ms/step, achieved bus GB/s (nccl-tests convention), fraction of 900 nominal / 770 measured}.  Times are
+    """{kind: calls/step, ms/step, achieved bus GB/s (nccl-tests convention), fraction of the 450 GB/s nominal}.  Times are
     CUDA-event spans of each call ON ITS STREAM, launch to completion: they include waiting for the slowest peer to arrive and the
     SM sharing with whatever compute runs beside the collective (side-stream collectives are hidden behind the GEMMs on purpose), so
-    these are in-step figures, below the stand-alone rates of profiles/r02_collectives_*gpu.jsonl.  A fused GEMM + collective is
-    judged against its own roofline: the slower of FLOPs / measured GEMM peak and NVLink bytes / 770 GB/s."""
+    these are in-step figures, below stand-alone collective rates.  A fused GEMM + collective is judged against its own roofline:
+    the slower of FLOPs / GEMM peak and NVLink bytes / 450 GB/s."""
     peak, _ = measured_peaks()
     out = {}
     for kind, recs in sorted(prof.items()):
@@ -293,10 +285,9 @@ def summarize_comm(prof, steps):
         flops = sum(r[3] for r in recs) if len(recs[0]) > 3 else 0.0
         gbs = nbytes / (ms * 1e-3) / 1e9 if ms > 0 else 0.0
         out[kind] = {"calls_per_step": round(len(recs) / steps, 1), "ms_per_step": round(ms / steps, 3), "bus_bytes_per_step": int(nbytes / steps),
-                     "bus_GBps": round(gbs, 1), "frac_of_900_nominal": round(gbs / NVLINK_NOMINAL_GBS, 3),
-                     "frac_of_770_measured": round(gbs / NVLINK_MEASURED_GBS, 3)}
+                     "bus_GBps": round(gbs, 1), "frac_of_450_nominal": round(gbs / NVLINK_NOMINAL_GBS, 3)}
         if flops > 0 and ms > 0:
-            bound_ms = sum(max(r[3] / (peak * 1e12), r[2] / (NVLINK_MEASURED_GBS * 1e9)) for r in recs) * 1e3
+            bound_ms = sum(max(r[3] / (peak * 1e12), r[2] / (NVLINK_NOMINAL_GBS * 1e9)) for r in recs) * 1e3
             out[kind].update({"tflops": round(flops / (ms * 1e-3) / 1e12, 1), "roofline_ms_per_step": round(bound_ms / steps, 3),
                               "frac_of_fused_roofline": round(bound_ms / ms, 3)})
     return out
@@ -329,7 +320,7 @@ def kernel_breakdown(step_fn, path, ms_per_step):
 
 
 def run_ours(opts):
-    os.environ.setdefault("PYTORCH_CUDA_ALLOC_CONF", "expandable_segments:True")   # 150+ GiB of long-lived state: avoid fragmentation
+    os.environ.setdefault("PYTORCH_CUDA_ALLOC_CONF", "expandable_segments:True")   # tens of GiB of long-lived state: avoid fragmentation
     import torch
     import torch.distributed as dist
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
@@ -350,7 +341,7 @@ def run_ours(opts):
             dist.barrier()
             dist.destroy_process_group()
         return
-    spath, strategy = strategy_for(world, opts.strategy)
+    spath, strategy = strategy_for(world, opts.model, opts.strategy)
     args, config, model = build_model(opts, strategy)
     be = get_backend()
     opt, _ = get_optimizer_and_param_scheduler(model, args)
@@ -435,6 +426,8 @@ def run_ours(opts):
     be.gemm_profile = []
     ms_res, launches, loss_res = timed(resident=True)
     prof, be.gemm_profile = be.gemm_profile, None
+    if opts.dump_outputs and rank == 0:
+        dump_outputs(opts.dump_outputs, model, loss_res)
     ms_e2e, _, loss_e2e = timed(resident=False)
     clocks = sampler.stop() if rank == 0 else None
     # one more step with every collective bracketed by CUDA events on its own stream: the in-step NVLink roofline
@@ -448,7 +441,6 @@ def run_ours(opts):
     gemm_ms = sum(rec[0].elapsed_time(rec[1]) for rec in prof)
     gemm_flops = sum(rec[2] for rec in prof)
     gemm_bytes = sum(rec[3] for rec in prof)
-    traffic, traffic_note = ncu_gemm_traffic(gemm_flops / max(1, len(prof)))
     peak, peak_src = measured_peaks()
     achieved = gemm_flops / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else 0.0
     h2d = 2 * (args.global_train_batch_size // dp_size) * config.max_position_embeddings * 8
@@ -461,7 +453,7 @@ def run_ours(opts):
                                                                        args.global_train_batch_size, os.path.basename(spath)),
                    "strategy": {k: strategy[k] for k in ("pp_deg", "chunks", "default_dp_type", "global_bsz") if k in strategy},
                    "tp": sorted(set(strategy["tp_sizes_enc"].split(","))), "checkpointed_layers": strategy.get("checkpoint", "").count("1"),
-                   "layers": config.num_hidden_layers, "l2": "inputs (16 GB of bf16 weights + activations per step) far exceed the 126 MB L2",
+                   "layers": config.num_hidden_layers, "l2": "inputs (GBs of bf16 weights + activations per step) far exceed the 50 MB L2",
                    "optimizer": ("AdamW fused into the gradient reduce-scatter kernel (fp32 shards)" if opts.optimizer == "fused"
                                  else "torch.optim.AdamW(fused=True) on fp32 flat shards"),
                    "collectives": "slim peer-memory kernels (128 thr x <=64 regs, one CTA per SM)%s; no NCCL on the path"
@@ -470,8 +462,8 @@ def run_ours(opts):
                 "d2h_bytes_per_step": 4 * max(1, strategy["chunks"]), "ms_per_step": round(ms_e2e / K, 3)},
         "gpu_launches": int(launches),
         "roofline": {"bound": "tensor", "achieved": round(achieved, 1), "peak": peak, "unit": "TFLOP/s",
-                     "frac": round(achieved / peak, 4) if peak else None, "traffic": traffic, "traffic_note": traffic_note,
-                     "algorithmic_bytes_per_launch_avg": gemm_bytes / max(1, len(prof)), "kernel": "gemm_bf16_kernel (tcgen05/TMEM/TMA)",
+                     "frac": round(achieved / peak, 4) if peak else None,
+                     "algorithmic_bytes_per_launch_avg": gemm_bytes / max(1, len(prof)), "kernel": "gemm_bf16_kernel (wgmma/TMA)",
                      "launches": len(prof), "kernel_ms_per_step": round(gemm_ms / K, 3), "share_of_step": round(gemm_ms / ms_res, 4),
                      "flops_per_launch_avg": gemm_flops / max(1, len(prof)), "peak_source": peak_src},
         "collectives_in_step": comm,
@@ -502,16 +494,44 @@ def run_ours(opts):
         dist.destroy_process_group()
 
 
+def dump_outputs(out_dir, model, loss):
+    """What the last timed step hands its caller: the loss and the updated fp32 master weights.  Every unit's weights are sampled
+    at up to DUMP_PER_UNIT positions drawn from a generator seeded by the unit's index, so the sample is the same from run to run;
+    the per-unit count shrinks with the number of units so that all samples together stay within DUMP_MAX_BYTES."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float("nan") if loss is None else loss], dtype=np.float64))
+    units = list(model.model.units)
+    per_unit = min(DUMP_PER_UNIT, DUMP_MAX_BYTES // 4 // max(1, len(units)))
+    for i, u in enumerate(units):
+        w = u.flat_param.detach()
+        g = torch.Generator().manual_seed(i)
+        idx = torch.randint(0, w.numel(), (min(per_unit, w.numel()),), generator=g).sort().values
+        np.save(os.path.join(out_dir, "weights_unit%03d.npy" % i), w[idx.to(w.device)].float().cpu().numpy())
+
+
+DUMP_PER_UNIT = 1 << 18      # fp32 samples per unit: 1 MiB each, 19 MiB for the 19 units of the Llama-3.2-1B shapes
+DUMP_MAX_BYTES = 63 << 20    # all weight samples together (the loss adds 8 bytes): under 64 MiB for any model
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # path legs: fixed-strategy runs of the collectives north_star names, one child process per rank and leg
 # ---------------------------------------------------------------------------------------------------------------------
 def leg_catalog(n):
     """name -> {model, strategy (Galvatron JSON, as the Search Engine would write it), tiny (the same strategy for the tiny model of
-    tests/_host_worker.py), expect (fused-kernel counters that must be > 0)}"""
-    def enc(v, layers=32):
+    tests/_host_worker.py), expect (fused-kernel counters that must be > 0)}
+
+    Memory per GPU (80 GB H100): B/parameter = 4 in the arena (bf16 weights + gradients of the parameters a rank holds unsharded) +
+    12 of fp32 master and Adam state (sharded over the ZeRO group).  The Llama legs use the headline model (1.50 B parameters, 16
+    layers): at most 24 GB of state per GPU under any of their strategies, plus the activations of one microbatch of 4 sequences of
+    8192 tokens split over TP/SP (<= 45 GB / N with the logits).  GPT-3 6.7B at N = 2 (PP2 only) holds 3.35 B parameters per GPU =
+    53.6 GB of state, so its layers are checkpointed there (activations of two 4096-token microbatches in flight: ~1 GB instead of
+    ~18 GB); at N >= 4 TP2 halves the state.  BERT-large (0.34 B) fits anywhere."""
+    def enc(v, layers=16):
         return ",".join([str(v)] * layers)
 
-    def strat(layers=32, **kw):
+    def strat(layers=16, **kw):
         d = {"pp_deg": 1, "tp_sizes_enc": enc(1, layers), "tp_consecutive_flags": enc(1, layers), "dp_types_enc": enc(0, layers),
              "use_sp": enc(0, layers), "checkpoint": enc(0, layers), "cp_sizes_enc": enc(1, layers), "global_bsz": 8, "chunks": 2,
              "pp_division": str(layers), "pipeline_type": "pipedream_flush", "default_dp_type": "zero2", "vtp": 1, "vsp": 0, "embed_sdp": 0}
@@ -522,27 +542,27 @@ def leg_catalog(n):
     spec = {"n_positions": 128 * n, "n_heads": heads, "n_kv_heads": max(2, n), "ffn_dim": 384, "dim": 128 if n < 8 else 256}
     legs = {}
     legs["tp%d_megatron_sp" % n] = dict(
-        model="llama3-8b", strategy=strat(tp_sizes_enc=enc(n), vtp=n, sequence_parallel=1),
+        model=MODEL, strategy=strat(tp_sizes_enc=enc(n), vtp=n, sequence_parallel=1),
         tiny=dict(global_tp_deg=n, vocab_tp=n, sequence_parallel=True, chunks=2, _spec=spec,
                   _env={"HGB_FUSE_GEMM_RS": "force", "HGB_FUSE_GEMM_AR": "force"}),
         expect=["ag_gemm", "gemm_rs"], what="C7/C8/C9: all-gather+GEMM and GEMM+reduce-scatter fused (layers.py:399-417,1061-1109,449-494)")
     legs["tp%d" % n] = dict(
-        model="llama3-8b", strategy=strat(tp_sizes_enc=enc(n), vtp=n, sequence_parallel=0),
+        model=MODEL, strategy=strat(tp_sizes_enc=enc(n), vtp=n, sequence_parallel=0),
         tiny=dict(global_tp_deg=n, vocab_tp=n, chunks=2, _spec=spec, _env={"HGB_FUSE_GEMM_AR": "force"}),
         expect=["gemm_ar"], what="C5/C6: GEMM+all-reduce fused, NVLS broadcast (layers.py:1110-1114, mappings_group.py:139)")
     legs["ulysses%d" % n] = dict(
-        model="llama3-8b", strategy=strat(tp_sizes_enc=enc(n), use_sp=enc(1), vtp=n, vsp=1, sequence_parallel=1),
+        model=MODEL, strategy=strat(tp_sizes_enc=enc(n), use_sp=enc(1), vtp=n, vsp=1, sequence_parallel=1),
         tiny=dict(global_tp_deg=n, vocab_tp=n, use_ulysses=True, sequence_parallel=True, chunks=2, _spec=spec),
         expect=[], what="C10: Ulysses all-to-all, q/k/v in one launch (transformer.py:1928-2062)")
     t2 = max(1, n // 2)
     legs["pp2_tp%d_1f1b" % t2] = dict(
-        model="llama3-8b", strategy=strat(pp_deg=2, tp_sizes_enc=enc(t2), vtp=t2, sequence_parallel=1 if t2 > 1 else 0, chunks=4,
-                                          pp_division="16,16"),
+        model=MODEL, strategy=strat(pp_deg=2, tp_sizes_enc=enc(t2), vtp=t2, sequence_parallel=1 if t2 > 1 else 0, chunks=4,
+                                          pp_division="8,8"),
         tiny=dict(pp_deg=2, global_tp_deg=t2, vocab_tp=t2, sequence_parallel=t2 > 1, chunks=4, pipeline_type="pipedream_flush",
                   global_train_batch_size=8, _spec=dict(spec, n_positions=128 * t2)),
         expect=[], what="C11: 1F1B-flush schedule, stage boundary = peer copy on a side stream + device flags (pipeline.py:375-701,1080-1257)")
     legs["zero3_ckpt_dp%d" % n] = dict(
-        model="llama3-8b", strategy=strat(dp_types_enc=enc(1), checkpoint=enc(1), global_bsz=2 * n, chunks=1, default_dp_type="zero3", embed_sdp=1),
+        model=MODEL, strategy=strat(dp_types_enc=enc(1), checkpoint=enc(1), global_bsz=2 * n, chunks=1, default_dp_type="zero3", embed_sdp=1),
         tiny=dict(sdp=1, global_checkpoint=1, embed_sdp=1, chunks=1, global_train_batch_size=2 * n, zero3_pool_slots=2),
         expect=[], what="C1/C2: ZeRO-3 all-gather (fwd + bwd re-gather) and reduce-scatter+AdamW per layer, pooled buffers, prefetch")
     # BASELINE.json config 3: GPT-3 6.7B, fixed strategy PP=2 x TP=2 x ZeRO-2 data parallel 2, 1F1B-flush (N = 8; PP2 x TP(N/2) below)
@@ -550,7 +570,8 @@ def leg_catalog(n):
     t3 = max(1, n // (2 * d3))
     legs["gpt-6.7b_pp2_tp%d_zero2dp%d_1f1b" % (t3, d3)] = dict(
         model="gpt-6.7b", seq=2048,
-        strategy=strat(pp_deg=2, tp_sizes_enc=enc(t3), vtp=t3, global_bsz=8 * d3, chunks=4, pp_division="16,16", default_dp_type="zero2"),
+        strategy=strat(layers=32, pp_deg=2, tp_sizes_enc=enc(t3, 32), vtp=t3, global_bsz=8 * d3, chunks=4, pp_division="16,16", default_dp_type="zero2",
+                       checkpoint=enc(1 if t3 == 1 else 0, 32)),
         tiny=dict(_family="gpt", pp_deg=2, global_tp_deg=t3, vocab_tp=t3, default_dp_type="zero2", chunks=4, pipeline_type="pipedream_flush",
                   global_train_batch_size=8, _spec=dict(n_positions=128 * t3, n_head=max(4, t3))),
         expect=[], what="BASELINE config 3: GPT-3 6.7B (gpt_hf family: LayerNorm, bias, GeLU, learned positions), PP2 x TP x ZeRO-2, 1F1B-flush")
@@ -565,11 +586,14 @@ def leg_catalog(n):
         expect=[], what="BASELINE config 4: BERT-large (bert_hf family: post-LN, non-causal attention with a padding mask, MLM head), "
                         "Ulysses all-to-all x data parallel, seq 8192")
     if n == 8:
-        legs["llama3-70b_zero3_ckpt_dp8"] = dict(
-            model="llama3-70b", strategy=strat(layers=80, dp_types_enc=enc(1, 80), checkpoint=enc(1, 80), global_bsz=8, chunks=1,
-                                               default_dp_type="zero3", embed_sdp=1),
-            tiny=None, expect=[], what="BASELINE config 5: Llama-3-70B SDP=8 ZeRO-3 + activation checkpointing (>= 0.40 s/step of NVLink time)")
-    if n == 8:      # config 5 before configs 3 and 4: if the wall-clock budget runs out, the later legs are the ones skipped
+        # BASELINE config 5 (Llama-3-70B SDP=8 ZeRO-3 + checkpointing) needs 12 B x 70.6 B / 8 = 106 GB of sharded fp32 state per GPU:
+        # it cannot fit 8 x 80 GB.  The same strategy on the 13B shapes of the reference's meta configs: 12 x 13.0 B / 8 = 19.5 GB
+        # of state + the ZeRO-3 pool (4 layers of bf16 weights, 3 of gradients: ~4.5 GB) + checkpointed activations (~3 GB at seq 8192).
+        legs["llama-13b_zero3_ckpt_dp8"] = dict(
+            model="llama-13b", strategy=strat(layers=40, dp_types_enc=enc(1, 40), checkpoint=enc(1, 40), global_bsz=8, chunks=1,
+                                              default_dp_type="zero3", embed_sdp=1),
+            tiny=None, expect=[], what="in place of BASELINE config 5 (70B does not fit 8 x 80 GB): 13B SDP=8 ZeRO-3 + activation checkpointing")
+    if n == 8:      # the ZeRO-3 run before configs 3 and 4: if the wall-clock budget runs out, the later legs are the ones skipped
         order = [k for k in legs if not k.startswith(("gpt-", "bert-"))] + [k for k in legs if k.startswith(("gpt-", "bert-"))]
         legs = {k: legs[k] for k in order}
     return legs
@@ -594,7 +618,7 @@ def run_path_legs(opts, rank, world, local):
     base_port = int(os.environ.get("MASTER_PORT", "29500")) + 11
     results = []
     for i, name in enumerate(names):
-        limit = 300.0 if "70b" in name else 170.0
+        limit = 300.0 if "13b" in name else 170.0
         decision = [None]
         if rank == 0:
             left = opts.total_budget_s - (time.time() - T_START)
@@ -746,8 +770,8 @@ def run_leg(opts):
 # ---------------------------------------------------------------------------------------------------------------------
 def cpu_reference_sample(opts, budget_s=25.0):
     """The CPU restatement of the reference path (oracle backend, all host threads) on a bounded sample of the workload:
-    Llama-3-8B shapes, embedding + lm_head + ONE and then TWO transformer layers, seq 1024, batch 1.  The two samples separate
-    the per-layer cost from the embedding/head cost; ``value`` is the full-depth (32-layer) tokens/s they imply -- an
+    the workload's shapes, embedding + lm_head + ONE and then TWO transformer layers, seq 1024, batch 1.  The two samples separate
+    the per-layer cost from the embedding/head cost; ``value`` is the full-depth tokens/s they imply -- an
     extrapolation that favours the CPU (seq 1024 instead of 8192: 8x less attention work per token), labelled as such, never a
     like-for-like 8B measurement (SURVEY 8d, BASELINE.md sec. 3)."""
     import torch
@@ -784,14 +808,15 @@ def cpu_reference_sample(opts, budget_s=25.0):
     t2, n2, _ = best_step(2, budget_s * 0.6)
     layer_s = max(t2 - t1, 0.05 * t1)
     other_s = max(t1 - layer_s, 0.0)
-    full_layers = 32
+    from hetu_galvatron_b200.llama_hf.meta_configs import _SPECS
+    full_layers = _SPECS[opts.model]["n_layers"]
     full_s = other_s + full_layers * layer_s
     return {"value": round(tok / full_s, 3), "unit": "tokens/s", "cores": cores, "kind": "port",
-            "sample": "oracle CPU restatement (fp32 compute, bf16 storage), Llama-3-8B shapes, seq 1024, batch 1: embedding + lm_head + "
+            "sample": "oracle CPU restatement (fp32 compute, bf16 storage), " + opts.model + " shapes, seq 1024, batch 1: embedding + lm_head + "
                       "1 layer (%d steps, median of the steps after the first %.2f s) and + 2 layers (%d steps, median %.2f s), intra-op threads "
                       "pinned to the host's cores -> %.2f s per layer, %.2f s for the rest; "
-                      "value = 1024 tokens / (rest + 32 layers) = extrapolated full-depth rate, NOT a like-for-like seq-8192 run"
-                      % (n1, t1, n2, t2, layer_s, other_s),
+                      "value = 1024 tokens / (rest + %d layers) = extrapolated full-depth rate, NOT a like-for-like seq-8192 run"
+                      % (n1, t1, n2, t2, layer_s, other_s, full_layers),
             "sample_tokens_per_s_1layer": round(tok / t1, 2)}
 
 

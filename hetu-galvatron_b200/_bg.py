@@ -2,7 +2,7 @@
 
 There is no CPU path: if ``libbg_galvatron.so`` is missing or fails to load, every use raises.  PyTorch is
 plumbing here (device memory, streams, the bootstrap exchange of IPC handles); the collectives themselves
-are the hand-written sm_100a kernels in ``csrc/``.
+are the hand-written sm_90a kernels in ``csrc/``.
 """
 import contextlib
 import ctypes

@@ -1,6 +1,6 @@
 """The execution backend the layer/runtime code talks to.
 
-Product = ``CudaBackend``: every method lands in a hand-written sm_100a kernel through the C ABI (``_bg``), or --
+Product = ``CudaBackend``: every method lands in a hand-written sm_90a kernel through the C ABI (``_bg``), or --
 for attention only -- in the flash-attn library the reference itself calls (transformer.py:495, SURVEY K3).
 There is no CPU implementation in this package: ``get_backend()`` raises when the extension or a GPU is missing.
 
@@ -38,16 +38,16 @@ def reset_backend():
 
 
 class CudaBackend:
-    """B200 backend: symmetric-memory communicator + fused kernels."""
+    """H100 backend: symmetric-memory communicator + fused kernels."""
 
-    name = "cuda-sm100a"
+    name = "cuda-sm90a"
     is_cuda = True
     FLAG_BYTES = 1 << 16
 
     def __init__(self, comm=None, arena_bytes=None, device=None):
         from ... import _bg
         if not torch.cuda.is_available():
-            raise _bg.BgError("hetu-galvatron_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _bg.BgError("hetu-galvatron_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.bg = _bg
         _bg.lib()
         self.rank, self.world = _world.get_rank(), _world.get_world_size()
@@ -108,6 +108,8 @@ class CudaBackend:
         self._staging = {}  # group ranks -> SymBuffer
         self._scratch = {}
         self.gemm_profile = None   # bench.py: list of (start_event, end_event, flops) while timing the dominant kernel
+        # RMSNorm / LayerNorm backward: one fp32 weight-gradient partial row per CTA, 3 CTAs of 256 threads x <= 76 registers per SM
+        self.norm_partials = 3 * torch.cuda.get_device_properties(self.device).multi_processor_count
 
     def close(self):
         if self.comm is not None:
@@ -435,7 +437,7 @@ class CudaBackend:
 
     # ---- math ops --------------------------------------------------------------------------------------------
     def gemm(self, a, b, layout, out=None, accumulate=False, m=None, n=None, k=None, addend=None):
-        """bf16 GEMM on tcgen05.  layout 'tn': a[M,K] b[N,K]; 'nn': a[M,K] b[K,N]; 'nt': a[K,M] b[K,N].
+        """bf16 GEMM on wgmma.  layout 'tn': a[M,K] b[N,K]; 'nn': a[M,K] b[K,N]; 'nt': a[K,M] b[K,N].
         ``addend`` [M,N]: out = A op B + addend in the epilogue (the residual add behind a projection, one rounding)."""
         code = {"tn": 0, "nn": 1, "nt": 2}[layout]
         if code == 2:
@@ -446,7 +448,7 @@ class CudaBackend:
         if out is None:
             out = torch.empty(m_, n_, dtype=torch.bfloat16, device=a.device)
         if a.dtype != torch.bfloat16 or b.dtype != torch.bfloat16 or out.dtype != torch.bfloat16:
-            raise self.bg.BgError("the B200 GEMM path is bf16-only (mixed_precision must be bf16)")
+            raise self.bg.BgError("the GEMM path is bf16-only (mixed_precision must be bf16)")
         assert a.is_contiguous() and b.is_contiguous() and out.is_contiguous()
         if m_ % 8 or n_ % 8 or k_ % 8:
             raise self.bg.BgError("GEMM dims (%d,%d,%d) must be multiples of 8" % (m_, n_, k_))
@@ -466,9 +468,8 @@ class CudaBackend:
             launch()
         return out
 
-    # measured (profiles/r01_fused_gemm_rs_4gpu_8gpu.jsonl, r02_fused_gemm_collectives_2gpu.jsonl, r02_fused_8gpu.jsonl): fusion pays when the
-    # GEMM lasts at least as long as the transfer of its output -- K = 3584 at p = 4: 0.226 vs 0.258 ms; below (K = 1792 at p = 8: 0.213 vs
-    # 0.197 unfused) the GEMM outruns NVLink and the fused kernel only adds its reducer tail
+    # fusion pays when the GEMM lasts at least as long as the transfer of its output; below that the GEMM outruns NVLink and the fused
+    # kernel only adds its reducer tail (thresholds from measurements on an earlier GPU; not re-measured on H100)
     FUSE_MIN_K = 3072
 
     def can_fuse_gemm_rs(self, m, n, group, k=None):
@@ -478,10 +479,10 @@ class CudaBackend:
         if k is not None and k < self.FUSE_MIN_K and os.environ.get("HGB_FUSE_GEMM_RS") != "force":
             return False
         buf = self._staging.get(tuple(group.ranks))
-        tiles = (m // p // 128) * ((n + 255) // 256)
+        tiles = (m // p // 128) * ((n + 127) // 128)
         return buf is not None and buf.data_bytes >= m * n * 2 and tiles * 4 <= self.FLAG_BYTES // 2
 
-    FUSE_AR_MIN_K = 2048   # as FUSE_MIN_K, for the fused GEMM + all-reduce (wins 9-14 % at K >= 2048, p = 2; loses 6-20 % at K <= 1792, p = 8)
+    FUSE_AR_MIN_K = 2048   # as FUSE_MIN_K, for the fused GEMM + all-reduce
 
     @staticmethod
     def _mnk(a, b, layout):
@@ -499,7 +500,7 @@ class CudaBackend:
         if k is not None and k < self.FUSE_AR_MIN_K and os.environ.get("HGB_FUSE_GEMM_AR") != "force":
             return False
         buf = self._staging.get(tuple(group.ranks))
-        tiles = (m // p // 128) * ((n + 255) // 256)
+        tiles = (m // p // 128) * ((n + 127) // 128)
         return buf is not None and buf.data_bytes >= m * n * 2 and tiles * 4 <= self.FLAG_BYTES // 2 // 2
 
     def gemm_all_reduce(self, a, b, layout, group):
@@ -539,7 +540,7 @@ class CudaBackend:
         return out, buf.u8[: m_ * k_ * 2].view(torch.bfloat16).view(m_, k_)
 
     def gemm_reduce_scatter(self, a, b, layout, group):
-        """[M, N] = A op B, reduce-scattered along M over ``group`` -> [M/p, N]: the tcgen05 GEMM's epilogue stores each
+        """[M, N] = A op B, reduce-scattered along M over ``group`` -> [M/p, N]: the wgmma GEMM's epilogue stores each
         partial tile into the owning rank's HBM and a tile reducer sums them as they land (GEMM + C8 in one operation)."""
         code = {"tn": 0, "nn": 1, "nt": 2}[layout]
         if code == 2:
@@ -566,7 +567,7 @@ class CudaBackend:
     def rmsnorm_bwd(self, dy, x, weight, rstd):
         x2, dy2 = x.reshape(-1, x.shape[-1]), dy.reshape(-1, x.shape[-1])
         dx = torch.empty_like(x2)
-        npart = min(444, max(1, x2.shape[0]))       # 3 CTAs of 256 threads x 76 registers per SM
+        npart = min(self.norm_partials, max(1, x2.shape[0]))
         dwp = torch.empty(npart, x2.shape[1], dtype=torch.float32, device=x.device)
         L = self.bg.lib()
         self.bg.check(L.bg_rmsnorm_bwd(_p(dy2), _p(x2), _p(weight), _p(rstd), _p(dx), _p(dwp), x2.shape[0], x2.shape[1], npart, _s()))
@@ -585,7 +586,7 @@ class CudaBackend:
     def layernorm_bwd(self, dy, x, weight, mean, rstd):
         x2, dy2 = x.reshape(-1, x.shape[-1]), dy.reshape(-1, x.shape[-1])
         dx = torch.empty_like(x2)
-        npart = min(444, max(1, x2.shape[0]))       # partial-sum rows (one per CTA; summed below)
+        npart = min(self.norm_partials, max(1, x2.shape[0]))       # partial-sum rows (one per CTA; summed below)
         dwp = torch.empty(npart, x2.shape[1], dtype=torch.float32, device=x.device)
         dbp = torch.empty_like(dwp)
         self.bg.check(self.bg.lib().bg_layernorm_bwd(_p(dy2), _p(x2), _p(weight), _p(mean), _p(rstd), _p(dx), _p(dwp), _p(dbp),
@@ -651,8 +652,7 @@ class CudaBackend:
 
     def attention(self, q, k, v, causal, softmax_scale, key_mask=None):
         """Attention is a LIBRARY call, as in the reference (transformer.py:495 calls flash-attn; K3 is not a collective and
-        is outside the hot-path scope).  On B200 the fastest library in the image is cuDNN's fused SDPA (tcgen05 kernels:
-        measured 1459 TFLOP/s fwd vs 370 for flash-attn 2's sm80-class kernels, profiles/r01_attention_libraries.jsonl), reached
+        is outside the hot-path scope).  The default is cuDNN's fused SDPA, reached
         through torch SDPA; HGB_ATTN=flash selects flash-attn 2.  q [b,s,n,d], k/v [b,s,ng,d] (GQA un-expanded).  Differentiable."""
         import torch.nn.functional as F
         from torch.nn.attention import SDPBackend, sdpa_kernel

@@ -3,7 +3,7 @@
 ``LinearWithGradAccumulationAndAsyncCommunication`` :375, ``ColumnParallelLinear`` :651, ``RowParallelLinear`` :927).
 
 What differs from the reference is where the bytes go, not the math:
-  * the GEMMs are the tcgen05 kernel (``backend.gemm``), and a GEMM whose result is about to be reduced writes it
+  * the GEMMs are the wgmma kernel (``backend.gemm``), and a GEMM whose result is about to be reduced writes it
     straight into the TP group's peer-visible staging buffer, so the all-reduce / reduce-scatter kernel pulls it over
     NVLink with no intermediate copy (reference: cuBLAS, then a separate NCCL kernel on the same stream);
   * the Megatron-SP all-gather lands in that staging buffer too and is consumed in place by the GEMM (reference: a
@@ -55,7 +55,7 @@ def _write_wgrad(weight, dy2d, x2d):
     if sink.dtype == dy2d.dtype:
         be.gemm(dy2d, x2d, "nt", out=sink, accumulate=unit.grad_started(weight))
     else:
-        # --reduce_in_fp32: the unsharded gradient buffer is fp32 (arguments.py:187); the tcgen05 GEMM writes bf16, so the wgrad
+        # --reduce_in_fp32: the unsharded gradient buffer is fp32 (arguments.py:187); the wgmma GEMM writes bf16, so the wgrad
         # goes through a bf16 tile buffer and the cast kernel accumulates it into the fp32 buffer
         tmp = be.gemm(dy2d, x2d, "nt")
         be.cast(tmp, sink, accumulate=unit.grad_started(weight))

@@ -4,7 +4,7 @@ ParallelAttention :512-900, Ulysses ``_SeqAllToAll`` / ``DistributedAttention`` 
 Llama family uses (``flash_attn.ops.rms_norm.RMSNorm``, LlamaModel_tensor_parallel.py:2,48).
 
 Data flow of one attention block (SBH activations, flash layout inside):
-    hidden [s,b,h] -> ColumnParallelLinear (tcgen05 GEMM, TP/SP comm in staging)           -> mixed [s,b,ng*(r+2)*hn]
+    hidden [s,b,h] -> ColumnParallelLinear (wgmma GEMM, TP/SP comm in staging)            -> mixed [s,b,ng*(r+2)*hn]
     -> ONE kernel: QKV split + RoPE + SBH->BSND relayout (K/V stay un-expanded for GQA)        -> q,k,v
     -> [Ulysses: ONE pull all-to-all for q,k,v with the head/seq transpose folded in]
     -> attention LIBRARY call (cuDNN SDPA; the reference calls flash-attn) -> [Ulysses: inverse all-to-all] -> context [s,b,np*hn]
@@ -247,7 +247,7 @@ def _attention(q, k, v, causal, scale, key_mask=None):
     if fn is None:
         out = None
     elif key_mask is None:
-        out = fn(q, k, v, causal, scale)                            # differentiable library call (cuDNN SDPA on B200)
+        out = fn(q, k, v, causal, scale)                            # differentiable library call (cuDNN SDPA)
     else:
         out = fn(q, k, v, causal, scale, key_mask)
     return out if out is not None else _FlashAttnFn.apply(q, k, v, causal, scale, key_mask)

@@ -1,14 +1,14 @@
 // bg_coll.cu -- the peer-memory collectives (SURVEY 2.3 rows C1-C3, C5-C10, C12-C14, C16) as SLIM kernels.
 //
 // Every cross-rank kernel here is 128 threads x <= 64 registers with no shared memory (8,192 registers per CTA), launched with
-// at most one CTA per SM ("comm_ctas", default 148).  The persistent tcgen05 GEMM CTA takes 40,960 registers and all of the
+// at most one CTA per SM ("comm_ctas", default 132).  The persistent wgmma GEMM CTA takes 36,864 registers and 193 KiB of the
 // shared memory of its SM, so up to three collectives (e.g. ZeRO-3's prefetch all-gather, the gradient reduce-scatter and a
 // tensor-parallel exchange) are resident BESIDE a running GEMM, and beside each other: a collective never has to wait for a
 // different kernel of its own rank to leave the SMs before its peers can see it arrive.  That removes the cross-rank deadlock
 // of round 1's 256-thread / 128-register kernels (two of them could not share an SM; rank A ran the all-gather and rank B the
 // reduce-scatter, each waiting for the peer kernel that could not become resident) without serialising the collectives on the
-// host.  Bandwidth: a peer load takes ~2,000 cycles (~1.8 us) over NVSwitch; 148 x 128 threads x 8 x 16 B = 2.4 MB in
-// flight covers 775 GB/s x 1.8 us = 1.4 MB (Little), so the slim kernels keep the NVLink pipe full.
+// host.  Bandwidth: a peer load takes ~2,000 cycles (~1.8 us) over NVSwitch; 132 x 128 threads x 8 x 16 B = 2.2 MB in
+// flight covers 450 GB/s x 1.8 us = 0.8 MB (Little), so the slim kernels keep the NVLink pipe full.
 //
 // With a multicast-bound buffer (NVLS, BG_CTX_VMM) the same kernels use the switch: multimem.st replicates an all-gather
 // store to every member (one store instead of p), multimem.ld_reduce returns the sum over the members (one load instead of p).
@@ -831,9 +831,9 @@ int bg_gemm_gather_launch(const void* a_local, const void* a_staged, const void*
                           int layout, int p, int me, const uint32_t* flags, uint32_t target, unsigned long long timeout_ns, int* err_dev,
                           cudaStream_t st);
 
-static size_t scatter_flag_count(long long m, long long n, int p) { return (size_t)((m / p + 127) / 128) * ((n + 255) / 256); }
+static size_t scatter_flag_count(long long m, long long n, int p) { return (size_t)((m / p + 127) / 128) * ((n + 127) / 128); }
 
-// C5/C8 fused: GEMM whose epilogue reduce-scatters over the group (tcgen05 tiles -> peer HBM -> tile reducer)
+// C5/C8 fused: GEMM whose epilogue reduce-scatters over the group (wgmma tiles -> peer HBM -> tile reducer)
 extern "C" int bg_gemm_reduce_scatter(bg_ctx_t c, int gid, int lane, const void* a, const void* b, long long m, long long n,
                                       long long k, int layout, const size_t* partial_offs, const size_t* flag_offs, void* out,
                                       void* stream) {

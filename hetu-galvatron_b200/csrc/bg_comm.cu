@@ -1,5 +1,5 @@
 // bg_comm.cu -- symmetric arena (cudaIpc or VMM), groups, device-side barrier, pipeline p2p and NVSwitch multicast setup.
-// The collective kernels themselves live in bg_coll.cu.  sm_100a; NVLink 5 / NVSwitch peer loads & stores, no NCCL.
+// The collective kernels themselves live in bg_coll.cu.  sm_90a; NVLink 4 / NVSwitch peer loads & stores, no NCCL.
 #include <math.h>
 #include <stdarg.h>
 #include <string.h>

@@ -1,4 +1,4 @@
-// Shared helpers for the bg_galvatron C-ABI library (sm_100a only).
+// Shared helpers for the bg_galvatron C-ABI library (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -31,14 +31,14 @@ int fail(int code, const char* fmt, ...);
     } while (0)
 
 struct Tunables {
-    long long comm_ctas = 148;     // CTAs of a cross-rank kernel (<= BG_MAX_CHANNELS): ONE slim CTA (128 thr x <= 64 regs) per SM
-    long long local_ctas = 148 * 8;  // CTAs of a purely local streaming kernel
+    long long comm_ctas = 132;     // CTAs of a cross-rank kernel (<= BG_MAX_CHANNELS): ONE slim CTA (128 thr x <= 64 regs) per SM
+    long long local_ctas = 132 * 8;  // CTAs of a purely local streaming kernel
     long long timeout_ms = 60000;  // device-side barrier timeout
     long long oneshot_bytes = 512 * 1024;
     long long nvls_min_bytes = 1 << 20;  // below this the peer-to-peer kernels win (latency)
     long long nvls_min_ranks = 4;        // groups smaller than this keep the peer-to-peer kernels (measured at p = 2: no gain from the switch)
-    long long nvls_gather = 0;     // all-gather stores through the switch (multimem.st) when the buffer is multicast-bound: measured at
-                                   // p = 8 NOT faster than p peer stores (616 vs 632 GB/s bus at 1 GiB, profiles/r02_collectives_8gpu.jsonl) -> off
+    long long nvls_gather = 0;     // all-gather stores through the switch (multimem.st) when the buffer is multicast-bound: off, p peer
+                                   // stores are the default path
     long long nvls_bcast = 1;      // the fused GEMM + all-reduce reducer writes a summed tile into every member's copy with ONE multimem.st
     long long nvls_reduce = 1;     // reduce-scatter loads are reduced in the switch (multimem.ld_reduce) when the buffer is multicast-bound
 };

@@ -1,12 +1,16 @@
-// bg_gemm.cu -- K1: bf16 GEMM on the 5th-gen tensor cores (tcgen05.mma, fp32 accumulators in TMEM, operands staged
+// bg_gemm.cu -- K1: bf16 GEMM on the Hopper tensor cores (wgmma.mma_async, fp32 accumulators in registers, operands staged
 // by TMA with 128-B swizzle), persistent, warp-specialised.  Replaces the torch.matmul -> cuBLAS calls of
 // galvatron/site_package/megatron/core/tensor_parallel/layers.py:417 (fwd), :462 (dgrad), :534 (wgrad).
 //
-//   tile            : BLOCK_M 128 x BLOCK_N 256 x BLOCK_K 64, one CTA per SM, UMMA 128x256x16 (cta_group::1)
-//   smem pipeline   : 4 stages x (A 16 KiB + B 32 KiB), full/empty mbarriers (TMA <-> MMA)
-//   TMEM            : 2 accumulator buffers x 256 columns (MMA of tile i+1 overlaps epilogue of tile i)
-//   warps           : 0 = TMA producer, 1 = MMA issuer, 2 = TMEM alloc, 4-7 = epilogue (TMEM -> regs -> swizzled smem
-//                     -> TMA store), 256 threads
+//   tile            : BLOCK_M 128 x BLOCK_N 128 x BLOCK_K 64, one CTA per SM; two consumer warpgroups, each issuing
+//                     wgmma m64n128k16 on its 64 rows of the tile (64 fp32 accumulators per thread)
+//   smem pipeline   : 5 stages x (A 16 KiB + B 16 KiB), full/empty mbarriers (TMA <-> wgmma)
+//   warps           : 0-7 = the two consumer warpgroups (wgmma, then the epilogue: registers -> swizzled smem -> TMA store),
+//                     8 = TMA producer; 288 threads.  The producer fills the stages of the next tile while the consumers run
+//                     the epilogue of this one.
+//   residency       : <= 136 registers per thread (288 x 136 = 39,168 per CTA) and 193 KiB of shared memory, so three slim
+//                     collective CTAs (128 threads x 64 registers, no shared memory, bg_coll.cu) stay resident beside a
+//                     running GEMM CTA
 //   layouts         : TN  C = A[M,K] * B[N,K]^T   (A, B K-major)
 //                     NN  C = A[M,K] * B[K,N]     (B MN-major: TMA boxes of 64 N-elements x 64 K-rows)
 //                     NT  C = A[K,M]^T * B[K,N]   (A, B MN-major)
@@ -19,15 +23,22 @@ using namespace bg;
 
 namespace {
 
-constexpr int BLOCK_M = 128, BLOCK_N = 256, BLOCK_K = 64, UMMA_K = 16;
-constexpr int kStages = 4, kAccStages = 2;
+constexpr int BLOCK_M = 128, BLOCK_N = 128, BLOCK_K = 64, WGMMA_K = 16;
+constexpr int kStages = 5;
 constexpr int kABytes = BLOCK_M * BLOCK_K * 2, kBBytes = BLOCK_N * BLOCK_K * 2, kStageBytes = kABytes + kBBytes;
 constexpr int kStoreCols = 64;                                 // columns per TMA store box (128 B)
 constexpr int kStoreBytes = BLOCK_M * kStoreCols * 2;          // 16 KiB per staging buffer
 constexpr int kNumStoreBufs = 2;
 constexpr int kSmemBytes = kStages * kStageBytes + kNumStoreBufs * kStoreBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-constexpr int kThreads = 256, kEpiThreads = 128;
-constexpr int kGroupM = 16;  // tile raster: 16 m-blocks share each sweep over n (L2 reuse)
+constexpr int kEpiThreads = 256, kThreads = kEpiThreads + 32;  // two consumer warpgroups + one producer warp
+constexpr int kProducerWarp = kEpiThreads / 32;
+constexpr int kMaxRegs = 136;
+constexpr int kWgOffset = 8192;  // smem offset of consumer warpgroup 1's operand A: 64 K-major rows, or the 2nd 64-wide M chunk
+constexpr int kGroupM = 16;      // tile raster: 16 m-blocks share each sweep over n (L2 reuse)
+static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KiB of shared memory per block");
+static_assert(kThreads * kMaxRegs + 3 * 128 * 64 <= 65536, "a GEMM CTA and three slim collective CTAs share an SM's registers");
+// H100: 228 KiB of shared memory per SM, of which the driver reserves 1 KiB per resident CTA (also for a CTA that uses none)
+static_assert(kSmemBytes + 1024 + 3 * 1024 <= 228 * 1024, "a GEMM CTA and three slim collective CTAs share an SM's shared memory");
 
 enum Layout { kTN = 0, kNN = 1, kNT = 2 };
 
@@ -66,30 +77,6 @@ __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.b
 template <int N>
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory"); }
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
@@ -97,23 +84,48 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout): start[0,14) lbo[16,30) sbo[32,46)
-// version=1 [46,48) layout_type[61,64) (2 = SWIZZLE_128B)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from touching the accumulators across an asynchronous wgmma (register dependences only)
+__device__ __forceinline__ void fence_acc(float* d) {
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x 128] (+)= A[64 x 16] * B[16 x 128], both operands in shared memory; kTransA / kTransB = 1 for an MN-major operand
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_m64n128(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(kTransA), "n"(kTransB));
+}
+
+// wgmma shared-memory matrix descriptor (cute::GMMA::GmmaDescriptor bit layout): start[0,14) lbo[16,30) sbo[32,46)
+// base_offset[49,52)=0 (stages are 1024-B aligned) layout_type[62,64) (1 = SWIZZLE_128B)
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
-}
-
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 [4,6)=1, a/b format BF16 [7,10)/[10,13)=1,
-// a_major bit 15, b_major bit 16 (0 = K-major, 1 = MN-major), n>>3 [17,23), m>>4 [24,29)
-__host__ __device__ constexpr uint32_t make_idesc(bool a_mn, bool b_mn) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-           ((uint32_t)(BLOCK_N >> 3) << 17) | ((uint32_t)(BLOCK_M >> 4) << 24);
 }
 
 struct TileCoord { int m, n; };
@@ -131,7 +143,7 @@ __device__ __forceinline__ TileCoord tile_of_virtual(int t, int m_blocks, int n_
     return {first_m + r % rows, r / rows};
 }
 
-// Fused GEMM + reduce-scatter (C5/C8): instead of storing C locally, the epilogue TMA-stores every finished 128x256 partial
+// Fused GEMM + reduce-scatter (C5/C8): instead of storing C locally, the epilogue TMA-stores every finished 128x128 partial
 // tile straight into the HBM of the rank that owns those rows (peer store over NVLink) and bumps that rank's per-tile
 // arrival counter; a small reducer kernel on the owner sums the p partials of a tile as soon as all have landed.  Transfer and
 // math overlap tile by tile; no NCCL, no separate collective pass over the full activation.
@@ -178,7 +190,7 @@ __device__ __forceinline__ TileCoord tile_of(int t, int m_blocks, int n_blocks, 
 }
 
 template <int kLayout, int kMode = kPlain>
-__global__ void __launch_bounds__(kThreads, 1) gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a,
+__global__ void __maxnreg__(kMaxRegs) gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                 const __grid_constant__ CUtensorMap map_b,
                                                                 const __grid_constant__ CUtensorMap map_c,
                                                                 const __nv_bfloat16* __restrict__ c_old, int M, int N, int K,
@@ -192,9 +204,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16_kernel(const __grid_con
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem_store + kNumStoreBufs * kStoreBytes);
     uint64_t* full_bar = bars;                       // [kStages]
     uint64_t* empty_bar = bars + kStages;            // [kStages]
-    uint64_t* tmem_full = bars + 2 * kStages;        // [kAccStages]
-    uint64_t* tmem_empty = tmem_full + kAccStages;   // [kAccStages]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + kAccStages);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m_blocks = (M + BLOCK_M - 1) / BLOCK_M, n_blocks = (N + BLOCK_N - 1) / BLOCK_N;
@@ -209,26 +218,17 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16_kernel(const __grid_con
         // registers before the GEMM CTA of that SM is resident.
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     }
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_c) : "memory");
-    }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < kStages; ++i) { mbar_init(smem_u32(full_bar + i), 1); mbar_init(smem_u32(empty_bar + i), 1); }
-        for (int i = 0; i < kAccStages; ++i) { mbar_init(smem_u32(tmem_full + i), 1); mbar_init(smem_u32(tmem_empty + i), kEpiThreads); }
+        // empty: one arrival per consumer warp once its wgmma reading the stage has retired
+        for (int i = 0; i < kStages; ++i) { mbar_init(smem_u32(full_bar + i), 1); mbar_init(smem_u32(empty_bar + i), kEpiThreads / 32); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         // ================= TMA producer =================
         if (elect_one()) {
             int stage = 0; uint32_t phase = 0;
@@ -281,73 +281,62 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16_kernel(const __grid_con
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        if (elect_one()) {
-            constexpr uint32_t idesc = make_idesc(kAMn, kBMn);
-            // K-major: 8-row groups 1024 B apart (SBO), K step 32 B inside the 128-B swizzle row
-            // MN-major: 64-element MN chunks BLOCK_K*128 B apart (LBO), 8-k-row groups 1024 B apart (SBO), K step 16 rows
-            constexpr uint32_t a_lbo = kAMn ? BLOCK_K * 128 : 0, b_lbo = kBMn ? BLOCK_K * 128 : 0;
-            constexpr uint32_t a_kstep = kAMn ? UMMA_K * 128 : UMMA_K * 2, b_kstep = kBMn ? UMMA_K * 128 : UMMA_K * 2;
-            int stage = 0; uint32_t phase = 0;
-            int acc = 0; uint32_t acc_phase = 0;
-            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-                mbar_wait(smem_u32(tmem_empty + acc), acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-                for (int kb = 0; kb < k_blocks; ++kb) {
-                    mbar_wait(smem_u32(full_bar + stage), phase);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem + stage * kStageBytes), sb = sa + kABytes;
+    } else {
+        // ================= consumers: wgmma main loop, then registers -> (+C) -> bf16 -> swizzled smem -> TMA store =================
+        const int wg = warp >> 2;                              // rows [64*wg, 64*wg+64) of the tile
+        const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // accumulator rows frag_row and frag_row + 8
+        const int frag_col = (lane & 3) * 2;                   // accumulator columns frag_col, +1 of every 8-column group
+        const bool issuer = threadIdx.x == 0;
+        // K-major: 8-row groups 1024 B apart (SBO), K step 32 B inside the 128-B swizzle row
+        // MN-major: 64-element MN chunks BLOCK_K*128 B apart (LBO), 8-k-row groups 1024 B apart (SBO), K step 16 rows
+        constexpr uint32_t a_lbo = kAMn ? BLOCK_K * 128 : 0, b_lbo = kBMn ? BLOCK_K * 128 : 0;
+        constexpr uint32_t a_kstep = kAMn ? WGMMA_K * 128 : WGMMA_K * 2, b_kstep = kBMn ? WGMMA_K * 128 : WGMMA_K * 2;
+        float acc[BLOCK_N / 2];
 #pragma unroll
-                    for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                        const uint64_t da = make_smem_desc(sa + k * a_kstep, a_lbo, 1024);
-                        const uint64_t db = make_smem_desc(sb + k * b_kstep, b_lbo, 1024);
-                        umma_bf16(d_tmem, da, db, idesc, (kb | k) != 0);
-                    }
-                    umma_commit(smem_u32(empty_bar + stage));  // frees the smem stage when these MMAs retire
-                    if (++stage == kStages) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(smem_u32(tmem_full + acc));          // accumulator complete -> epilogue
-                if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else if (warp >= 4) {
-        // ================= epilogue: TMEM -> registers -> (+C) -> bf16 -> swizzled smem -> TMA store =================
-        const int ew = warp - 4;                      // == warp % 4: TMEM lanes [32*ew, 32*ew+32)
-        const int row = ew * 32 + lane;               // row inside the tile
-        const bool issuer = threadIdx.x == 4 * 32;
-        int acc = 0; uint32_t acc_phase = 0;
+        for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+        int stage = 0; uint32_t phase = 0;
         int buf = 0;
         uint32_t* prev_flag = nullptr;                // fused scatter: arrival counter of the tile whose stores are in flight
         for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
             const TileCoord tc = tile_of<kMode>(t, m_blocks, n_blocks, sp);
-            mbar_wait(smem_u32(tmem_full + acc), acc_phase);
-            tc_fence_after();
-#pragma unroll 1
+            int prev_stage = 0;
+            for (int kb = 0; kb < k_blocks; ++kb) {
+                mbar_wait(smem_u32(full_bar + stage), phase);
+                const uint32_t sa = smem_u32(smem + stage * kStageBytes) + wg * kWgOffset;
+                const uint32_t sb = smem_u32(smem + stage * kStageBytes) + kABytes;
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BLOCK_K / WGMMA_K; ++k) {
+                    const uint64_t da = make_smem_desc(sa + k * a_kstep, a_lbo, 1024);
+                    const uint64_t db = make_smem_desc(sb + k * b_kstep, b_lbo, 1024);
+                    wgmma_m64n128<kAMn ? 1 : 0, kBMn ? 1 : 0>(acc, da, db, (kb | k) != 0);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                               // k-block kb-1's wgmmas have retired: its stage is free
+                if (kb > 0 && lane == 0) mbar_arrive(smem_u32(empty_bar + prev_stage));
+                prev_stage = stage;
+                if (++stage == kStages) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            fence_acc(acc);
+            if (lane == 0) mbar_arrive(smem_u32(empty_bar + prev_stage));
+#pragma unroll
             for (int c = 0; c < BLOCK_N / kStoreCols; ++c) {
                 const int n0 = tc.n * BLOCK_N + c * kStoreCols;
                 if (n0 >= N) break;  // whole chunk out of bounds (uniform across the CTA)
-                uint32_t v[64];
-                const uint32_t taddr = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(acc * BLOCK_N + c * kStoreCols);
-                tmem_ld32(taddr, v);
-                tmem_ld32(taddr + 32, v + 32);
-                tmem_ld_wait();
-                if (c == BLOCK_N / kStoreCols - 1 || n0 + kStoreCols >= N) {
-                    // last TMEM read of this tile: hand the accumulator back to the MMA warp
-                    tc_fence_before();
-                    mbar_arrive(smem_u32(tmem_empty + acc));
-                }
+                float* v = acc + c * (kStoreCols / 2);         // 8 column groups x {row, row + 8} x 2 columns
                 if (accumulate) {
-                    const long long grow = (long long)tc.m * BLOCK_M + row;
-                    if (grow < M) {
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            if (n0 + j * 8 < N) {
-                                float o[8];
-                                unpack8(*reinterpret_cast<const uint4*>(c_old + grow * N + n0 + j * 8), o);
+                    for (int h = 0; h < 2; ++h) {
+                        const long long grow = (long long)tc.m * BLOCK_M + frag_row + 8 * h;
+                        if (grow < M) {
 #pragma unroll
-                                for (int e = 0; e < 8; ++e) v[j * 8 + e] = __float_as_uint(__uint_as_float(v[j * 8 + e]) + o[e]);
+                            for (int j = 0; j < 8; ++j) {
+                                if (n0 + j * 8 < N) {
+                                    const float2 o = bf2_to_f2(*reinterpret_cast<const uint32_t*>(c_old + grow * N + n0 + j * 8 + frag_col));
+                                    v[j * 4 + 2 * h] += o.x;
+                                    v[j * 4 + 2 * h + 1] += o.y;
+                                }
                             }
                         }
                     }
@@ -357,14 +346,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16_kernel(const __grid_con
                 epi_bar_sync();
                 uint8_t* sbuf = smem_store + buf * kStoreBytes;
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    uint4 pk;
-                    pk.x = f2_to_bf2(__uint_as_float(v[j * 8 + 0]), __uint_as_float(v[j * 8 + 1]));
-                    pk.y = f2_to_bf2(__uint_as_float(v[j * 8 + 2]), __uint_as_float(v[j * 8 + 3]));
-                    pk.z = f2_to_bf2(__uint_as_float(v[j * 8 + 4]), __uint_as_float(v[j * 8 + 5]));
-                    pk.w = f2_to_bf2(__uint_as_float(v[j * 8 + 6]), __uint_as_float(v[j * 8 + 7]));
-                    // 128-B swizzle: 16-B chunk j of row r lives at chunk (j ^ (r & 7))
-                    *reinterpret_cast<uint4*>(sbuf + row * 128 + ((j ^ (row & 7)) << 4)) = pk;
+                for (int h = 0; h < 2; ++h) {
+                    const int row = frag_row + 8 * h;
+#pragma unroll
+                    for (int j = 0; j < 8; ++j)   // 128-B swizzle: 16-B chunk j of row r lives at chunk (j ^ (r & 7))
+                        *reinterpret_cast<uint32_t*>(sbuf + row * 128 + ((j ^ (row & 7)) << 4) + frag_col * 2) =
+                            f2_to_bf2(v[j * 4 + 2 * h], v[j * 4 + 2 * h + 1]);
                 }
                 fence_proxy_async();
                 epi_bar_sync();
@@ -381,7 +368,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16_kernel(const __grid_con
             }
             if constexpr (kScatter) {
                 if (issuer) {
-                    // Publish the PREVIOUS tile: every bulk group except this tile's (<= 4 chunks) has completed, so its peer
+                    // Publish the PREVIOUS tile: every bulk group except this tile's (<= 2 chunks) has completed, so its peer
                     // stores are done -- no stall on this tile's NVLink latency.
                     if (prev_flag != nullptr) {
                         asm volatile("cp.async.bulk.wait_group %0;" ::"n"(BLOCK_N / kStoreCols) : "memory");
@@ -392,7 +379,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16_kernel(const __grid_con
                     prev_flag = sp.flags[owner] + ((row0 - owner * sp.rows_per_rank) / BLOCK_M) * n_blocks + tc.n;
                 }
             }
-            if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
         }
         if (issuer) {
             tma_store_wait_all<0>();
@@ -403,13 +389,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16_kernel(const __grid_con
                 }
             }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
     }
 }
 
@@ -481,7 +460,7 @@ static int make_ab_maps(CUtensorMap* ma, CUtensorMap* mb, const void* a, const v
     // A: TN/NN stored [M][K] (K-major: box 64 K x 128 rows); NT stored [K][M] (MN-major: box 64 M x 64 K-rows)
     int rc = layout == kNT ? make_map(ma, a, k, m, 64, BLOCK_K) : make_map(ma, a, m, k, BLOCK_K, BLOCK_M);
     if (rc) return rc;
-    // B: TN stored [N][K] (box 64 K x 256 rows); NN/NT stored [K][N] (box 64 N x 64 K-rows)
+    // B: TN stored [N][K] (box 64 K x BLOCK_N rows); NN/NT stored [K][N] (box 64 N x 64 K-rows)
     return layout == kTN ? make_map(mb, b, n, k, BLOCK_K, BLOCK_N) : make_map(mb, b, k, n, 64, BLOCK_K);
 }
 

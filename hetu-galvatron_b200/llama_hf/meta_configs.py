@@ -16,6 +16,9 @@ _SPECS = {
     # BASELINE.json configs (no meta file shipped by the reference; SURVEY 8 shapes)
     "llama3-8b": dict(dim=4096, ffn_dim=14336, n_heads=32, n_kv_heads=8, n_layers=32, norm_eps=1e-5, vocab_size=128256,
                       n_positions=8192, multiple_of=256),
+    # Llama-3.2-1B shapes (untied embeddings): the flagship on one 80 GB GPU, where Llama-3-8B's AdamW state alone does not fit
+    "llama3.2-1b": dict(dim=2048, ffn_dim=8192, n_heads=32, n_kv_heads=8, n_layers=16, norm_eps=1e-5, vocab_size=128256,
+                        n_positions=8192, multiple_of=256),
     "llama3-70b": dict(dim=8192, ffn_dim=28672, n_heads=64, n_kv_heads=8, n_layers=80, norm_eps=1e-5, vocab_size=128256,
                        n_positions=8192, multiple_of=256),
 }

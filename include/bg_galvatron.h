@@ -1,5 +1,5 @@
 /*
- * bg_galvatron.h -- C ABI of the B200-native hot path behind Hetu-Galvatron's per-layer strategy API.
+ * bg_galvatron.h -- C ABI of the H100-native hot path behind Hetu-Galvatron's per-layer strategy API.
  *
  * The reference (PKU-DAIR/Hetu-Galvatron v2.4.1) has no FFI at this seam: every per-layer collective is a
  * torch.distributed (ProcessGroupNCCL) call made from Python.  Each entry point below names the reference
@@ -45,7 +45,7 @@ enum bg_err {
 /* ---- library ------------------------------------------------------------------------------------------ */
 int bg_abi_version(void);
 const char* bg_last_error(void);                       /* thread-local message of the last failing call */
-/* "comm_ctas" (CTAs of a cross-rank kernel, default 148 = one 128-thread / <=64-register CTA per SM), "local_ctas", "timeout_ms",
+/* "comm_ctas" (CTAs of a cross-rank kernel, default 132 = one 128-thread / <=64-register CTA per SM), "local_ctas", "timeout_ms",
  * "oneshot_bytes", "nvls_min_bytes" (multicast paths above this size), "nvls_min_ranks" (... and from this group size on), "nvls_gather" [0] / "nvls_reduce" [1]
  * (multimem.st for all-gather / multimem.ld_reduce for reduce-scatter on multicast-bound buffers; defaults from the p = 8 measurement),
  * "nvls_bcast" [1] (the fused GEMM + all-reduce writes a reduced tile to every member with one multimem.st) */
@@ -184,7 +184,7 @@ int bg_ce_sumexp(const void* logits, int dtype, const long long* target, const f
 int bg_ce_bwd(void* logits, int dtype, const long long* target, const float* rowmax, const float* sum2,
               const float* grad_loss, long long rows, long long vocab_local, long long vocab_start, void* stream);
 
-/* ---- GEMM (K1): bf16 x bf16 -> fp32 accumulate in TMEM -> bf16, tcgen05 + TMA ------------------------------ */
+/* ---- GEMM (K1): bf16 x bf16 -> fp32 accumulate in registers -> bf16, wgmma + TMA -------------------------- */
 /* C[M,N] (+)= A op B.  layout: 0 = "TN" C = A[M,K] * B[N,K]^T (forward, layers.py:417);
  * 1 = "NN" C = A[M,K] * B[K,N] (dgrad, layers.py:462); 2 = "NT" C = A[K,M]^T * B[K,N] (wgrad, layers.py:534). */
 int bg_gemm_bf16(const void* a, const void* b, void* c, long long m, long long n, long long k, int layout,
@@ -194,7 +194,7 @@ int bg_gemm_bf16(const void* a, const void* b, void* c, long long m, long long n
 int bg_gemm_bf16_add(const void* a, const void* b, void* c, const void* addend, long long m, long long n, long long k, int layout,
                      void* stream);
 
-/* C5/C8 fused with K1: C = A op B is computed in 128x256 tcgen05 tiles and REDUCE-SCATTERED along M over the group inside
+/* C5/C8 fused with K1: C = A op B is computed in 128x128 wgmma tiles and REDUCE-SCATTERED along M over the group inside
  * the same operation -- every finished partial tile is TMA-stored into the owning rank's arena (peer HBM over NVLink) and
  * counted there; a tile reducer on the owner -- launched into the same stream as the GEMM's programmatic dependent, so it
  * runs beside the GEMM CTAs once all of them are resident -- sums the p partials as they land and writes out[M/p, N].

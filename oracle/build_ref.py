@@ -1,21 +1,20 @@
-"""TEST / TOOLING INFRASTRUCTURE (oracle/): builds oracle/_ref/ from the reference's own sources where they lie under
-/root/reference (never copied into the repo; oracle/_ref/ is git-ignored but travels to the GPU box).
+"""TEST / TOOLING INFRASTRUCTURE (oracle/): builds oracle/_ref/ from the reference's own sources in a checkout of the upstream
+Hetu-Galvatron tree (never copied into the repo; oracle/_ref/ is git-ignored).
 
 The hot path of the reference is Python over torch/NCCL -- there is no C/C++ source OF THE PATH to compile (DESIGN.md section 5).
 The one C++ file the reference ships is the Search Engine's dynamic-programming core, csrc/dp_core.cpp (pybind11); it is what
-`scripts/search_strategy.py` runs, unmodified, to produce the strategies bench.py loads, so it is built here too.
-Called by __graft_entry__.build(); a no-op when /root/reference is absent (GPU box)."""
+`scripts/search_strategy.py` runs, unmodified, to search strategies from measured profiles, so it is built here.
+Called by scripts/search_strategy.py with the checkout's path; a no-op when the source is absent."""
 import os
 import subprocess
 import sys
 import sysconfig
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
 
 
-def build():
-    src = os.path.join(REF, "csrc", "dp_core.cpp")
+def build(ref):
+    src = os.path.join(ref, "csrc", "dp_core.cpp")
     if not os.path.exists(src):
         print("[oracle/build_ref] %s not present: nothing to build" % src)
         return None
@@ -32,4 +31,4 @@ def build():
 
 
 if __name__ == "__main__":
-    build()
+    build(sys.argv[1])

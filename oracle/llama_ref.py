@@ -17,7 +17,7 @@ tests/core/test_tp.py:60-121).  Follows, line by line:
 accumulate); torch.float32/float64 gives the exact-math answer.  Parity status: PINNED.  The reference ships no golden tensors
 (SURVEY 8c), so the pins are outputs of the reference run here: (1) HF ``LlamaForCausalLM`` in fp64 -- the model the reference's own
 tests compare with (tests/test_oracle_llama.py: per-token loss 2e-6, gradients 1e-5); (2) the unmodified reference RUNTIME executed on
-B200s under 7 strategies (oracle/ref_runtime/run_ref.py -> tests/golden/ref_runtime/*.json): the host runtime, whose every strategy is
+GPUs under 7 strategies (oracle/ref_runtime/run_ref.py -> tests/golden/ref_runtime/*.json): the host runtime, whose every strategy is
 checked against this file, reproduces the reference's losses over 3 Adam steps to 4e-5 and its all-rank gradient norm to 6e-4
 (tests/test_ref_runtime_parity.py).
 """

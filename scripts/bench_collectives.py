@@ -5,7 +5,7 @@
 For each message size and collective: the slim peer-to-peer kernel, the same kernel on the multicast path (NVLS: multimem.st /
 multimem.ld_reduce, when the fabric supports it) and the torch.distributed (NCCL) sequence the reference issues at the same call
 site -- all CUDA-event timed (median launch, max over ranks), bus bandwidth by the nccl-tests convention (AG/RS/A2A (p-1)/p*N,
-AR 2(p-1)/p*N) against 900 GB/s nominal / 770 GB/s measured peer copy, and a result comparison (bit-exact for data movement,
+AR 2(p-1)/p*N) against 450 GB/s nominal (H100 NVLink 4, per direction), and a result comparison (bit-exact for data movement,
 bf16 tolerance for reductions).  JSON lines on rank 0; COLLECTIVES_OK / COLLECTIVES_FAIL last."""
 import argparse
 import json

@@ -8,7 +8,7 @@ galvatron/utils/config_utils.py:59-91,108-137):
     overlap_coefficient.json                           {"overlap_coe": x}
 NVSwitch gives strided and consecutive groups the same bandwidth, so consec_0 == consec_1.
 
-    python scripts/emit_hardware_profile.py profiles/r01_collectives_2gpu_v2.jsonl [more.jsonl ...] --out configs/hardware_b200
+    python scripts/emit_hardware_profile.py collectives_2gpu.jsonl [more.jsonl ...] --out <dir for search_strategy.py --hardware-dir>
 """
 import argparse
 import json
@@ -19,7 +19,7 @@ import os
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("tables", nargs="+")
-    ap.add_argument("--out", default="configs/hardware_b200")
+    ap.add_argument("--out", required=True)
     ap.add_argument("--gpus-per-node", type=int, default=8)
     opts = ap.parse_args()
     rows = []

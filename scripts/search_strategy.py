@@ -1,16 +1,16 @@
 #!/usr/bin/env python
-"""Run the reference's UNMODIFIED Search Engine (galvatron/core/search_engine + csrc/dp_core.cpp) on B200 profiles and
-emit the strategy JSONs bench.py loads (configs/galvatron_config_llama3-8b_<N>gpus.json).
+"""Run the reference's UNMODIFIED Search Engine (galvatron/core/search_engine + csrc/dp_core.cpp) on profiles measured on the
+target GPU and emit Galvatron strategy JSONs for Llama-3-8B shapes (galvatron_config_llama3-8b_<N>gpus.json under --out-root).
 
-Only runs in the build container (needs /root/reference); the emitted JSONs are committed.  Inputs:
-  * computation profile  : per-layer / head forward ms per sample measured with THIS runtime on B200 (profiles/, see
-                           --layer-ms/--other-ms), static mode (search_engine.py:123-131)
+Needs a checkout of the upstream Hetu-Galvatron sources (--reference).  Inputs:
+  * computation profile  : per-layer / head forward ms per sample measured with THIS runtime on the target GPU
+                           (--layer-ms/--other-ms), static mode (search_engine.py:123-131)
   * memory profile       : analytic from the model shapes in the reference's units (MB; parameter_size = fp32 MB,
                            model_states = 4 x parameter_size, cost_model.py:118), activations from the saved-tensor list
                            of our layer (DESIGN.md section 3)
   * hardware profile     : all-reduce / p2p bandwidth and sp_time tables measured with OUR collectives
                            (scripts/bench_collectives.py) -- NVSwitch makes consecutive and strided groups identical
-The search DP core is compiled from /root/reference/csrc/dp_core.cpp into oracle/_ref/ (never copied into the repo).
+The search DP core is compiled from <reference>/csrc/dp_core.cpp into oracle/_ref/ (never copied into the repo).
 """
 import argparse
 import glob
@@ -21,16 +21,15 @@ import sys
 import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
 
 
-def build_dp_core():
-    """oracle/build_ref.py owns the recipe (also run by __graft_entry__.build())."""
+def build_dp_core(ref):
+    """oracle/build_ref.py owns the recipe."""
     import importlib.util
     spec = importlib.util.spec_from_file_location("_oracle_build", os.path.join(ROOT, "oracle", "build_ref.py"))
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
-    so = mod.build()
+    so = mod.build(ref)
     if so is None:
         raise SystemExit("the reference sources are not present: the Search Engine cannot run here")
     return os.path.dirname(so)
@@ -84,25 +83,27 @@ def hardware_profiles(bus_gbs, p2p_gbs, latency_ms):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--layer-ms", type=float, default=4.4, help="forward ms of one layer for one 8192-token sample (measured)")
-    ap.add_argument("--other-ms", type=float, default=7.6, help="forward ms of embedding + lm_head + loss for one sample (measured)")
-    ap.add_argument("--bus-gbs", type=float, default=600.0)
-    ap.add_argument("--p2p-gbs", type=float, default=700.0)
+    ap.add_argument("--reference", required=True, help="checkout of the upstream Hetu-Galvatron sources")
+    ap.add_argument("--layer-ms", type=float, required=True, help="forward ms of one layer for one 8192-token sample (measured)")
+    ap.add_argument("--other-ms", type=float, required=True, help="forward ms of embedding + lm_head + loss for one sample (measured)")
+    ap.add_argument("--bus-gbs", type=float, required=True, help="collective bus GB/s (scripts/bench_collectives.py)")
+    ap.add_argument("--p2p-gbs", type=float, required=True, help="peer-copy GB/s")
     ap.add_argument("--latency-ms", type=float, default=0.02)
-    ap.add_argument("--memory-gb", type=int, default=170)
+    ap.add_argument("--memory-gb", type=int, default=64, help="memory the engine may plan with (80 GB H100 less the arena and headroom)")
     ap.add_argument("--seq", type=int, default=8192)
     ap.add_argument("--gpus", type=int, nargs="*", default=[1, 2, 4, 8])
-    ap.add_argument("--hardware-dir", default=os.path.join(ROOT, "configs", "hardware_b200"),
+    ap.add_argument("--hardware-dir", default=None,
                     help="measured tables from scripts/emit_hardware_profile.py (used when present; else the latency+bandwidth model)")
     ap.add_argument("--recompute-activations", action="store_true",
                     help="memory profile of the runtime's --recompute_activations mode (NOT the bench default; measure before use)")
-    ap.add_argument("--out-root", default=os.path.join(ROOT, "configs"),
+    ap.add_argument("--out-root", required=True,
                     help="where search_profiles/ and searched/ are written (tests point this at a temp dir)")
     ap.add_argument("--debug-memory", action="store_true", help="print the engine's per-layer memory model for the dp-only strategy")
     opts = ap.parse_args()
 
-    dp_dir = build_dp_core()
-    sys.path[:0] = [dp_dir, os.path.join(ROOT, "oracle", "ref_shim"), REF, os.path.join(REF, "galvatron", "site_package"), REF]
+    ref = os.path.abspath(opts.reference)
+    dp_dir = build_dp_core(ref)
+    sys.path[:0] = [dp_dir, os.path.join(ROOT, "oracle", "ref_shim"), ref, os.path.join(ref, "galvatron", "site_package"), ref]
     import warnings
     warnings.filterwarnings("ignore")
     from galvatron.core.search_engine.search_engine import GalvatronSearchEngine
@@ -119,8 +120,8 @@ def main():
         ar, p2p, ov, sp = hardware_profiles(opts.bus_gbs, opts.p2p_gbs, opts.latency_ms)
         measured = {k: os.path.join(opts.hardware_dir, f) for k, f in (
             ("ar", "allreduce_bandwidth_1nodes_8gpus_per_node.json"), ("p2p", "p2p_bandwidth_1nodes_8gpus_per_node.json"),
-            ("ov", "overlap_coefficient.json"), ("sp", "sp_time_1nodes_8gpus_per_node.json"))}
-        if all(os.path.exists(f) for f in measured.values()):   # tables measured with OUR collectives on 2/4/8 B200s
+            ("ov", "overlap_coefficient.json"), ("sp", "sp_time_1nodes_8gpus_per_node.json"))} if opts.hardware_dir else {}
+        if measured and all(os.path.exists(f) for f in measured.values()):   # tables measured with OUR collectives
             ar.update(json.load(open(measured["ar"])))
             p2p.update(json.load(open(measured["p2p"])))
             ov = json.load(open(measured["ov"]))

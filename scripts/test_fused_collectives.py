@@ -5,7 +5,7 @@
   gemm_all_reduce       C5  row-parallel forward, C6 column-parallel dgrad          (layers.py:1110-1114, mappings_group.py:139)
   all_gather_gemm       C7  column-parallel forward under SP, row-parallel dgrad    (layers.py:399-417, mappings_group.py:243-258)
 
-Roofline of a fused op (B200_PROFILING.md): the slower of FLOPs / measured GEMM peak and NVLink bytes / 770 GB/s measured.
+Roofline of a fused op: the slower of FLOPs / GEMM peak and NVLink bytes / 450 GB/s (H100 SXM data-sheet figures).
     torchrun --nproc-per-node N --master-addr 127.0.0.1 scripts/test_fused_collectives.py
 """
 import json
@@ -21,7 +21,7 @@ from hetu_galvatron_b200.core.runtime.backend import get_backend, reset_backend 
 from hetu_galvatron_b200.core.runtime.comm_groups import CommGroup  # noqa: E402
 
 BF = torch.bfloat16
-GEMM_PEAK_TFLOPS, NVLINK_GBS = 1321.9, 770.0      # MEASURED_PEAKS.json sustained cuBLAS bf16; measured peer copy
+GEMM_PEAK_TFLOPS, NVLINK_GBS = 989.0, 450.0       # H100 SXM data sheet: dense bf16, NVLink 4 per direction
 
 
 def timed(fn, iters=10, warm=3):

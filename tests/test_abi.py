@@ -44,14 +44,14 @@ def test_exports_match_nm(bg):
     assert set(_declared_symbols()) <= exported
 
 
-def test_kernels_are_blackwell_native(bg):
-    """SASS evidence (B200_PROFILING.md): tcgen05.mma -> UTC*MMA, tcgen05.ld -> LDTM, TMA -> UTMALDG/UTMASTG."""
+def test_kernels_are_hopper_native(bg):
+    """SASS evidence: wgmma.mma_async -> HGMMA, TMA -> UTMALDG/UTMASTG, all for sm_90a."""
     sass = subprocess.run(["cuobjdump", "-sass", bg.LIB_PATH], capture_output=True, text=True).stdout
     if not sass:
         pytest.skip("cuobjdump unavailable")
-    for mnemonic in ("UTCHMMA", "LDTM", "UTMALDG", "UTMASTG"):
+    for mnemonic in ("HGMMA", "UTMALDG", "UTMASTG"):
         assert mnemonic in sass, mnemonic
-    assert "sm_100a" in sass
+    assert "sm_90a" in sass
 
 
 def test_errors_are_return_codes(bg):
@@ -62,7 +62,7 @@ def test_errors_are_return_codes(bg):
     assert L.bg_group_create(None, None, 0, None) == -1
     with pytest.raises(bg.BgError):
         bg.check(L.bg_arena_alloc(None, 16, None))
-    assert bg.get_tunable("comm_ctas") == 148      # one slim CTA per SM
+    assert bg.get_tunable("comm_ctas") == 132      # one slim CTA per SM
 
 
 def test_c_mirror_of_group_builder_matches_goldens(bg):

@@ -1,6 +1,6 @@
 """GPU parity of the peer-memory collectives (through the C ABI) against oracle/collectives_ref.py.
 
-One B200 is enough: ``BgComm.local_world(n)`` creates n virtual ranks (n contexts, n arenas) on the device and
+One H100 is enough: ``BgComm.local_world(n)`` creates n virtual ranks (n contexts, n arenas) on the device and
 every rank's kernel runs on its own stream, so the real cross-rank protocol (device barriers, peer loads/stores
 through the peer-pointer table) is what executes.  Integer/byte-moving paths are checked bit-exact; reductions
 against the fp64 "exact" oracle (fp32 accumulate => 1e-6) and against the reference-order oracle (bf16 rounding).

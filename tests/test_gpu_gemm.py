@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05/TMEM/TMA GEMM (through the C ABI) against torch fp32 matmul of the same bf16 inputs.
+"""GPU parity of the wgmma/TMA GEMM (through the C ABI) against torch fp32 matmul of the same bf16 inputs.
 Covers the three layouts of the Megatron linear layer (layers.py:417 fwd TN, :462 dgrad NN, :534 wgrad NT), ragged
 edges (TMA zero-fill / clipping), accumulate mode, and the Llama-3-8B shapes of BASELINE config (2)."""
 import os

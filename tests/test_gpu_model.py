@@ -68,7 +68,7 @@ def _torchrun(n, script, port, env=None, timeout=600):
 @pytest.mark.parametrize("n", [2, 4, 8])
 def test_fused_gemm_collectives(n):
     """GEMM + reduce-scatter, GEMM + all-reduce and all-gather + GEMM on n real GPUs at the Llama-3-8B tensor-parallel shapes vs
-    cuBLAS + NCCL (reductions) / the plain tcgen05 GEMM on the gathered operand (bit-exact)."""
+    cuBLAS + NCCL (reductions) / the plain wgmma GEMM on the gathered operand (bit-exact)."""
     _need(n)
     out = _torchrun(n, "test_fused_collectives.py", 29800 + n)
     assert out.returncode == 0 and "FUSED_OK" in out.stdout, out.stdout[-3000:] + out.stderr[-3000:]

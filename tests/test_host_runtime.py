@@ -102,7 +102,7 @@ WORLD4 = {
 # reference test sets it (test_hybrid.py:45).
 _HYBRID = dict(tp_consecutive_flags="1,1,1,1", use_sp="0,1,0,1", checkpoint="0,0,1,1", global_bsz=32,
                pipeline_type="pipedream_flush", default_dp_type="zero2")
-# (ffn 384: a tensor-parallel degree of 8 leaves K = 48 for the row-parallel GEMM -- the tcgen05 kernel wants multiples of 8)
+# (ffn 384: a tensor-parallel degree of 8 leaves K = 48 for the row-parallel GEMM -- the wgmma kernel wants multiples of 8)
 _SPEC8 = {"n_heads": 8, "n_kv_heads": 8, "n_layers": 4, "ffn_dim": 384}
 def _redistributed(tp, vtp, sp):
     """tests/core/test_redistributed.py:49-69,141-146: zero2, no checkpointing, per-layer tp lists that force a relocation between
