@@ -1,5 +1,5 @@
 """Micro-benchmarks of the C-ABI kernels on one GPU (CUDA events, warm-up, L2-exceeding inputs).
-Usage: python scripts/bench_kernels.py [gemm] [cast] [coll]  -> JSON lines on stdout."""
+Usage: python scripts/bench_kernels.py [gemm] [cast] [ops] [attn]  -> JSON lines on stdout."""
 import json
 import os
 import sys
@@ -25,21 +25,84 @@ def timeit(fn, iters=10, warm=3):
     return s.elapsed_time(e) / iters
 
 
+# The 15 GEMMs of one microbatch of the flagship workload (Llama-3.2-1B shapes, seq 8192): (layout, M, N, K, epilogue).
+# epilogue: None, "addend" (the residual add of the row-parallel projections) or "acc" (wgrad of microbatches 2..8).
+FLAGSHIP_GEMMS = [
+    (0, 8192, 3072, 2048, None), (0, 8192, 2048, 2048, "addend"), (0, 8192, 16384, 2048, None),
+    (0, 8192, 2048, 8192, "addend"), (0, 8192, 128256, 2048, None),
+    (1, 8192, 2048, 3072, None), (1, 8192, 2048, 2048, None), (1, 8192, 2048, 16384, None), (1, 8192, 8192, 2048, None),
+    (1, 8192, 2048, 128256, None),
+    (2, 3072, 2048, 8192, "acc"), (2, 2048, 2048, 8192, "acc"), (2, 16384, 2048, 8192, "acc"), (2, 2048, 8192, 8192, "acc"),
+    (2, 128256, 2048, 8192, "acc"),
+]
+
+
 def gemm():
-    shapes = [(0, 8192, 6144, 4096), (0, 8192, 4096, 4096), (0, 8192, 28672, 4096), (0, 8192, 4096, 14336),
-              (1, 8192, 4096, 6144), (1, 8192, 4096, 28672), (2, 6144, 4096, 8192), (2, 28672, 4096, 8192),
-              (2, 4096, 14336, 8192), (0, 8192, 128256, 4096), (0, 8192, 8192, 8192)]
-    for layout, m, n, k in shapes:
-        a = torch.randn((k, m) if layout == 2 else (m, k), device="cuda").to(BF)
-        b = torch.randn((n, k) if layout == 0 else (k, n), device="cuda").to(BF)
-        c = torch.empty(m, n, device="cuda", dtype=BF)
-        t_mine = timeit(lambda: bg.gemm_bf16(a, b, c, m, n, k, layout))
-        at, bt = (a.t() if layout == 2 else a), (b.t() if layout == 0 else b)
-        t_ref = timeit(lambda: torch.matmul(at, bt, out=c))
+    """The flagship GEMMs, ours and cuBLAS (torch) interleaved round by round, on input sets rotated so that their sum exceeds
+    the 50 MB L2.  operand_TBps = the A and B bytes the CTAs load from L2 into shared memory (tiles x k-blocks x 32 KiB) over
+    the kernel time."""
+    import math
+    import subprocess
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True)
+    print(json.dumps({"nvidia_smi": q.stdout.strip()}), flush=True)
+    rounds = 5
+    for layout, m, n, k, epi in FLAGSHIP_GEMMS:
+        set_bytes = 2 * (m * k + n * k + (2 if epi == "addend" else 1) * m * n)
+        sets = []
+        for _ in range(max(1, math.ceil(200e6 / set_bytes))):
+            a = torch.randn((k, m) if layout == 2 else (m, k), device="cuda").to(BF)
+            b = torch.randn((n, k) if layout == 0 else (k, n), device="cuda").to(BF)
+            c = torch.randn(m, n, device="cuda").to(BF)
+            add = torch.randn(m, n, device="cuda").to(BF) if epi == "addend" else None
+            sets.append((a, b, c, add))
         fl = 2.0 * m * n * k
-        print(json.dumps({"bench": "gemm", "layout": layout, "m": m, "n": n, "k": k, "ms": round(t_mine, 4),
-                          "tflops": round(fl / t_mine / 1e9, 1), "cublas_ms": round(t_ref, 4),
-                          "cublas_tflops": round(fl / t_ref / 1e9, 1)}), flush=True)
+        iters = max(4, math.ceil(0.1 * 4e14 / fl))      # ~100 ms per timed window
+
+        def ours(s):
+            a, b, c, add = s
+            if epi == "addend":
+                bg.gemm_bf16_add(a, b, c, add, m, n, k, layout)
+            else:
+                bg.gemm_bf16(a, b, c, m, n, k, layout, accumulate=epi == "acc")
+
+        def cublas(s):
+            a, b, c, add = s
+            at, bt = (a.t() if layout == 2 else a), (b.t() if layout == 0 else b)
+            if epi == "addend":
+                torch.addmm(add, at, bt, out=c)
+            elif epi == "acc":
+                c.addmm_(at, bt)
+            else:
+                torch.matmul(at, bt, out=c)
+
+        def window(fn):
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record()
+            for i in range(iters):
+                fn(sets[i % len(sets)])
+            e.record()
+            torch.cuda.synchronize()
+            return s.elapsed_time(e) / iters
+
+        arms = {"cublas": cublas, "ours": ours}
+        times = {name: [] for name in arms}
+        for fn in arms.values():        # warm-up: module load, cuBLAS heuristics
+            window(fn)
+        for _ in range(rounds):
+            for name, fn in arms.items():
+                times[name].append(window(fn))
+        rec = {"bench": "gemm", "layout": "TN NN NT".split()[layout], "m": m, "n": n, "k": k, "epilogue": epi}
+        for name, ts in times.items():
+            t = sorted(ts)[rounds // 2]
+            rec[name + "_ms"] = round(t, 4)
+            rec[name + "_tflops"] = round(fl / t / 1e9, 1)
+            rec[name + "_spread_pct"] = round(100 * (max(ts) - min(ts)) / t, 1)
+        tiles_kblocks = -(-m // 128) * -(-n // 128) * -(-k // 64)
+        rec["ours_operand_TBps"] = round(tiles_kblocks * 32768 / rec["ours_ms"] / 1e9, 2)
+        print(json.dumps(rec), flush=True)
+        del sets
+        torch.cuda.empty_cache()
 
 
 def cast():
