@@ -8,7 +8,8 @@ from ..core.runtime.pipeline import PipeSequential
 from ..core.runtime.tensor_parallel import (gather_from_tensor_model_parallel_region_group,
                                             linear_with_grad_accumulation_and_async_allreduce,
                                             scatter_to_sequence_parallel_region_group, vocab_parallel_cross_entropy)
-from ..gpt_hf.GPTModel_sequential import _seq_slice, _size
+from ..core.runtime.tensor_parallel.random import check_probability
+from ..gpt_hf.GPTModel_sequential import _embedding_dropout, _seq_slice, _size
 
 
 class BertWordEmbedding_(nn.Module):
@@ -51,6 +52,7 @@ class BertEmbeddings_(nn.Module):
         self.vocab_sp = args.vocab_sp
         if self.vocab_sp:
             self.seq_start_index, self.seq_end_index = _seq_slice(args, self.sp_group)
+        self.dropout_p = check_probability(getattr(args, "hidden_dropout", 0.0), "hidden_dropout")     # after the LayerNorm, :100-102
 
     def forward(self, input_ids, token_type_ids=None, position_ids=None, attention_mask=None, labels=None):
         if position_ids is None:
@@ -66,7 +68,7 @@ class BertEmbeddings_(nn.Module):
         embeddings = embeddings.transpose(0, 1).contiguous()                  # [b, s, h] -> [s, b, h]
         if self.sequence_parallel:
             embeddings = scatter_to_sequence_parallel_region_group(embeddings, self.tp_group)
-        return embeddings
+        return _embedding_dropout(self, embeddings)
 
 
 class BertLayers_(nn.Module):

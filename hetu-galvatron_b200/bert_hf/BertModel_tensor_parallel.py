@@ -6,7 +6,8 @@ from torch import nn
 from ..core.runtime.arguments import get_args
 from ..core.runtime.tensor_parallel import (AttnMaskType, AttnType, ColumnParallelLinear, LayerNorm, ParallelAttention, ParallelMLP,
                                             VocabParallelEmbedding)
-from ..gpt_hf.GPTModel_tensor_parallel import _megatron_sp, core_transformer_config_from_args
+from ..core.runtime.tensor_parallel.random import SITE_ATTENTION, SITE_MLP, bias_dropout_add, site
+from ..gpt_hf.GPTModel_tensor_parallel import _megatron_sp, _seq_rank, core_transformer_config_from_args
 
 
 class BertAttention_tp(nn.Module):
@@ -21,9 +22,15 @@ class BertAttention_tp(nn.Module):
                                            tp_group=self.tp_group, sp_group=self.sp_group, use_ulysses=self.use_ulysses, device="meta")
         self.LayerNorm = LayerNorm(config.hidden_size, eps=config.layer_norm_eps, device="meta",
                                    sequence_parallel=_megatron_sp(args, tp_group))
+        # attention_dropout on the attention-block output, as the reference (:29-36)
+        self.dropout_p, self.site = mconf.attention_dropout, site(layer_number + 1, SITE_ATTENTION)
+        self.seq_rank = _seq_rank(args, tp_group, sp_group)
 
     def forward(self, hidden_states, attention_mask):
         residual = hidden_states
+        if self.dropout_p > 0.0 and self.training:
+            out, bias = self.attention(hidden_states, attention_mask)
+            return self.LayerNorm(bias_dropout_add(out, bias, residual, self.dropout_p, self.site, self.seq_rank * out.shape[0]))
         hidden_states, bias = self.attention(hidden_states, attention_mask, residual=residual)   # + residual in the GEMM epilogue
         if bias is not None:
             hidden_states = hidden_states + bias
@@ -31,7 +38,7 @@ class BertAttention_tp(nn.Module):
 
 
 class BertMLP_tp(nn.Module):
-    def __init__(self, config, tp_group=None):
+    def __init__(self, config, tp_group=None, layer_number=0, sp_group=None):
         super().__init__()
         args = get_args()
         mconf = core_transformer_config_from_args(args)
@@ -39,9 +46,14 @@ class BertMLP_tp(nn.Module):
         self.mlp = ParallelMLP(mconf, tp_group=self.tp_group, device="meta")
         self.LayerNorm = LayerNorm(config.hidden_size, eps=config.layer_norm_eps, device="meta",
                                    sequence_parallel=_megatron_sp(args, tp_group))
+        self.dropout_p, self.site = mconf.hidden_dropout, site(layer_number + 1, SITE_MLP)       # :48-55
+        self.seq_rank = _seq_rank(args, tp_group, sp_group)
 
     def forward(self, hidden_states):
         residual = hidden_states
+        if self.dropout_p > 0.0 and self.training:
+            out, bias = self.mlp(hidden_states)
+            return self.LayerNorm(bias_dropout_add(out, bias, residual, self.dropout_p, self.site, self.seq_rank * out.shape[0]))
         hidden_states, bias = self.mlp(hidden_states, residual=residual)
         if bias is not None:
             hidden_states = hidden_states + bias
@@ -52,7 +64,7 @@ class BertLayer_tp(nn.Module):
     def __init__(self, config, layer_number, tp_group=None, sp_group=None):
         super().__init__()
         self.attention = BertAttention_tp(config, layer_number, tp_group, sp_group)
-        self.mlp = BertMLP_tp(config, tp_group)
+        self.mlp = BertMLP_tp(config, tp_group, layer_number, sp_group)
         self.idx = layer_number
 
     def forward(self, hidden_states, attention_mask=None):

@@ -18,6 +18,9 @@ def config_from_meta(model_type):
         num_key_value_heads=p["num_attention_heads"], intermediate_size=p.get("intermediate_size") or 4 * h, vocab_size=p["vocab_size"],
         max_position_embeddings=p["max_position_embeddings"], type_vocab_size=p.get("type_vocab_size", 2),
         layer_norm_eps=p.get("layer_norm_eps", 1e-12), hidden_act=p.get("hidden_act", "gelu"),
+        # BertConfig's dropouts (0.1 each in HF; 0 in the shipped specs here, see arguments.hidden_dropout)
+        hidden_dropout_prob=float(p.get("hidden_dropout_prob", 0.0)),
+        attention_probs_dropout_prob=float(p.get("attention_probs_dropout_prob", 0.0)),
         model_name=model_type if isinstance(model_type, str) else "custom")
 
 
@@ -37,4 +40,6 @@ def set_model_config(config, args, overwrite_args=True):
         args.vocab_size = config.vocab_size
         mult = getattr(args, "make_vocab_size_divisible_by", 128) * max(1, getattr(args, "vocab_tp", 1))
         args.padded_vocab_size = (config.vocab_size + mult - 1) // mult * mult
+        # config_utils.py:57-58,68-69 (overwrite_megatron_args)
+        args.hidden_dropout, args.attention_dropout = config.hidden_dropout_prob, config.attention_probs_dropout_prob
     return config

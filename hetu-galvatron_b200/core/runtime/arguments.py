@@ -13,7 +13,14 @@ _ARGS = None
 DEFAULTS = dict(
     initialize_on_meta=0,                # :23
     global_train_batch_size=32,          # :29
-    dropout_prob=0.0,                    # :30 default 0.1; the random-data scripts force 0 (config_utils.py:98-99)
+    dropout_prob=0.0,                    # :30 default 0.1; read by no layer here (the GPT / BERT families take hidden_dropout /
+                                         # attention_dropout below); > 0 still makes the checkpoint wrapper preserve the RNG state
+    # megatron's names; the GPT / BERT families set them from the HF config (resid_pdrop / attn_pdrop, hidden_dropout_prob /
+    # attention_probs_dropout_prob) as the reference's overwrite_megatron_args does.  Deviation on purpose: 0 by default (the
+    # reference gets 0.1 from the HF config defaults), so no run changes unless it asks for dropout.  Llama keeps 0 (as the reference).
+    hidden_dropout=0.0,                  # embedding output and MLP-block output (megatron --hidden-dropout)
+    attention_dropout=0.0,               # attention probabilities AND the attention-block output (megatron --attention-dropout;
+                                         # the reference applies it at both, GPTModel_tensor_parallel.py:31-39)
     adam_weight_decay=0.01,              # :32
     pp_deg=2,                            # :52
     global_cp_deg=1,                     # :60

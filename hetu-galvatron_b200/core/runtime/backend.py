@@ -607,6 +607,34 @@ class CudaBackend:
                                                  1 if tanh_form else 0, _s()))
         return dx.view_as(x)
 
+    def dropout_add_fwd(self, x, bias, residual, p, seed, iteration, site, seq_base, sample_base):
+        """y = residual + keep * scale * (x + bias) on an SBH tensor x [s_loc, b_loc, h] whose rows are tokens seq_base.. of samples
+        sample_base.. (mask: include/bg_galvatron.h).  bias [h] (bf16 / fp32) and residual (x's shape) may be None."""
+        s, b, h = x.shape
+        x = x.contiguous()
+        y = torch.empty_like(x)
+        if residual is not None:
+            residual = residual.contiguous()
+            assert residual.shape == x.shape and residual.dtype == x.dtype
+        bcode = self.bg.dtype_code(bias.dtype) if bias is not None else 0
+        self.bg.check(self.bg.lib().bg_dropout_add_fwd(_p(x), _p(bias) if bias is not None else None, bcode,
+                                                       _p(residual) if residual is not None else None, _p(y), s * b, h, b,
+                                                       int(seq_base), int(sample_base), float(p), int(seed), int(iteration),
+                                                       int(site), _s()))
+        return y
+
+    def dropout_bwd(self, dy, p, seed, iteration, site, seq_base, sample_base, with_bias):
+        """-> (dx = keep * scale * dy, dbias = its fp32 column sums or None), the mask regenerated from the same coordinates."""
+        s, b, h = dy.shape
+        dy = dy.contiguous()
+        dx = torch.empty_like(dy)
+        npart = min(self.norm_partials, max(1, s * b))
+        dbp = torch.empty(npart, h, dtype=torch.float32, device=dy.device) if with_bias else None
+        self.bg.check(self.bg.lib().bg_dropout_bwd(_p(dy), _p(dx), _p(dbp) if dbp is not None else None, npart, s * b, h, b,
+                                                   int(seq_base), int(sample_base), float(p), int(seed), int(iteration), int(site),
+                                                   _s()))
+        return dx, (dbp.sum(0) if dbp is not None else None)
+
     def swiglu_fwd(self, gate_up):
         rows, two_f = gate_up.reshape(-1, gate_up.shape[-1]).shape
         y = torch.empty(gate_up.shape[:-1] + (two_f // 2,), dtype=gate_up.dtype, device=gate_up.device)
@@ -650,10 +678,13 @@ class CudaBackend:
         # the reference casts cos/sin to the activation dtype before applying them (apply_rotary_pos_emb)
         return torch.cos(freqs).to(dtype).float().contiguous(), torch.sin(freqs).to(dtype).float().contiguous()
 
-    def attention(self, q, k, v, causal, softmax_scale, key_mask=None):
+    def attention(self, q, k, v, causal, softmax_scale, key_mask=None, dropout_p=0.0):
         """Attention is a LIBRARY call, as in the reference (transformer.py:495 calls flash-attn; K3 is not a collective and
         is outside the hot-path scope).  The default is cuDNN's fused SDPA, reached
-        through torch SDPA; HGB_ATTN=flash selects flash-attn 2.  q [b,s,n,d], k/v [b,s,ng,d] (GQA un-expanded).  Differentiable."""
+        through torch SDPA; HGB_ATTN=flash selects flash-attn 2.  q [b,s,n,d], k/v [b,s,ng,d] (GQA un-expanded).  Differentiable.
+        ``dropout_p`` > 0: dropout on the attention probabilities (transformer.py:443-503), drawn from torch's CUDA generator (the
+        caller runs this under the model-parallel RNG tracker); SDPA may then pick the flash or memory-efficient kernel instead of
+        cuDNN's."""
         import torch.nn.functional as F
         from torch.nn.attention import SDPBackend, sdpa_kernel
         if key_mask is not None:
@@ -664,13 +695,16 @@ class CudaBackend:
             bias.masked_fill_(~key_mask.bool()[:, None, None, :], float("-inf"))
             with sdpa_kernel([SDPBackend.CUDNN_ATTENTION, SDPBackend.EFFICIENT_ATTENTION, SDPBackend.MATH]):
                 o = F.scaled_dot_product_attention(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), attn_mask=bias,
-                                                   scale=softmax_scale, enable_gqa=k.shape[2] != q.shape[2])
+                                                   dropout_p=dropout_p, scale=softmax_scale, enable_gqa=k.shape[2] != q.shape[2])
             return o.transpose(1, 2)
         if self.attn_impl != "cudnn":
             return None
-        with sdpa_kernel([SDPBackend.CUDNN_ATTENTION]):
+        backends = [SDPBackend.CUDNN_ATTENTION]
+        if dropout_p > 0.0:
+            backends += [SDPBackend.FLASH_ATTENTION, SDPBackend.EFFICIENT_ATTENTION]
+        with sdpa_kernel(backends):
             o = F.scaled_dot_product_attention(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), is_causal=causal,
-                                               scale=softmax_scale, enable_gqa=k.shape[2] != q.shape[2])
+                                               dropout_p=dropout_p, scale=softmax_scale, enable_gqa=k.shape[2] != q.shape[2])
         return o.transpose(1, 2)
 
     def attention_prefix(self, q, k, v, softmax_scale):
@@ -681,17 +715,18 @@ class CudaBackend:
         from flash_attn import flash_attn_func
         return flash_attn_func(q, k, v, dropout_p=0.0, softmax_scale=softmax_scale, causal=True)
 
-    def attention_fwd(self, q, k, v, causal, softmax_scale):
-        """flash-attn 2 library call (the reference's choice); used when HGB_ATTN=flash."""
+    def attention_fwd(self, q, k, v, causal, softmax_scale, key_mask=None, dropout_p=0.0):
+        """flash-attn 2 library call (the reference's choice); used when HGB_ATTN=flash.  Its backward replays ``rng``."""
         from flash_attn.flash_attn_interface import _flash_attn_forward
-        out, lse, _, rng = _flash_attn_forward(q, k, v, 0.0, softmax_scale, causal=causal, window_size_left=-1,
+        assert key_mask is None, "the flash-attn path takes no padding mask"
+        out, lse, _, rng = _flash_attn_forward(q, k, v, dropout_p, softmax_scale, causal=causal, window_size_left=-1,
                                                window_size_right=-1, softcap=0.0, alibi_slopes=None, return_softmax=False)
         return out, lse, rng
 
-    def attention_bwd(self, dout, q, k, v, out, lse, causal, softmax_scale, rng):
+    def attention_bwd(self, dout, q, k, v, out, lse, causal, softmax_scale, rng, dropout_p=0.0):
         from flash_attn.flash_attn_interface import _flash_attn_backward
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
-        _flash_attn_backward(dout.contiguous(), q, k, v, out, lse, dq, dk, dv, 0.0, softmax_scale, causal, -1, -1, 0.0, None,
+        _flash_attn_backward(dout.contiguous(), q, k, v, out, lse, dq, dk, dv, dropout_p, softmax_scale, causal, -1, -1, 0.0, None,
                              False, rng_state=rng)
         return dq, dk, dv
 

@@ -18,6 +18,7 @@ from .comm_groups import gen_comm_groups
 from .hybrid_parallel_config import (check_hp_config, get_chunks, hp_config_whole_model, layer_shapes_dtypes_whole_model,
                                      mixed_precision_dtype)
 from .parallel import finalize_pools, wrap_modules_relocation
+from .tensor_parallel import random as dropout_random
 
 
 class GalvatronModel(nn.Module):
@@ -38,6 +39,11 @@ class GalvatronModel(nn.Module):
             loss_func = self.fake_loss_func
             assert isinstance(batch, (tuple, list))
             batch = [batch, [self.fake_tensor(batch[0])]]
+        # dropout coordinates of this step: the iteration, and the global index of this rank's first sample (the batch is split
+        # contiguously over the data-parallel ranks of the vocabulary rows)
+        dp = getattr(self, "vtp_data_group", None)
+        local = next((t.shape[0] for t in batch[0] if torch.is_tensor(t)), 0)
+        dropout_random.begin_iteration(getattr(args, "seed", 0), self.iter, (dp.rank_in_group() if dp is not None else 0) * local)
         if args.pp_deg > 1:
             if args.pipeline_type == "gpipe":
                 loss = model.gpipe_forward(batch, loss_func, **kwargs)

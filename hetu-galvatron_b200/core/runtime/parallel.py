@@ -29,6 +29,7 @@ import torch.nn as nn
 
 from .backend import get_backend
 from .redistribute import fused_split_allgather
+from .tensor_parallel import random as dropout_random
 
 _DP_TYPES = ("ddp", "zero2", "zero3")
 
@@ -483,11 +484,14 @@ class _CheckpointFn(torch.autograd.Function):
         ctx.is_tensor = [torch.is_tensor(t) for t in inputs]
         ctx.others = [t for t in inputs if not torch.is_tensor(t)]
         # dropout inside the layer must draw the same masks when it is recomputed (checkpoint_wrapper preserves the RNG state,
-        # torch/utils/checkpoint.py); only captured when dropout is on -- the random-data scripts run with 0
+        # torch/utils/checkpoint.py); only captured when dropout is on.  The hidden-state masks need the microbatch's dropout
+        # context (the backward may run under another microbatch's), attention-probability dropout the default generator AND the
+        # model-parallel tracker's streams.
         ctx.rng = None
         if wrapper.preserve_rng:
             dev = next((t.device for t in inputs if torch.is_tensor(t) and t.is_cuda), None)
-            ctx.rng = (torch.get_rng_state(), dev, torch.cuda.get_rng_state(dev) if dev is not None else None)
+            ctx.rng = (torch.get_rng_state(), dev, torch.cuda.get_rng_state(dev) if dev is not None else None,
+                       dropout_random.get_context(), dropout_random.get_rng_tracker().get_states())
         with torch.no_grad():
             out = wrapper.module(*inputs, **kwargs)
         return out
@@ -506,17 +510,23 @@ class _CheckpointFn(torch.autograd.Function):
             else:
                 inputs.append(others.pop(0))
         if ctx.rng is not None:
-            cpu_state, dev, cuda_state = ctx.rng
-            now = (torch.get_rng_state(), torch.cuda.get_rng_state(dev) if dev is not None else None)
+            cpu_state, dev, cuda_state, drop_ctx, tracker_states = ctx.rng
+            tracker = dropout_random.get_rng_tracker()
+            now = (torch.get_rng_state(), torch.cuda.get_rng_state(dev) if dev is not None else None, dropout_random.get_context(),
+                   tracker.get_states())
             torch.set_rng_state(cpu_state)
             if dev is not None:
                 torch.cuda.set_rng_state(cuda_state, dev)
+            dropout_random.set_context(drop_ctx)
+            tracker.set_states(tracker_states)
         with torch.enable_grad():
             out = wrapper.module(*inputs, **ctx.kwargs)
         if ctx.rng is not None:
             torch.set_rng_state(now[0])
             if dev is not None:
                 torch.cuda.set_rng_state(now[1], dev)
+            dropout_random.set_context(now[2])
+            tracker.set_states(now[3])
         outs = out if isinstance(out, (tuple, list)) else (out,)
         pairs = [(o, g) for o, g in zip(outs, grads) if torch.is_tensor(o) and o.requires_grad and g is not None]
         torch.autograd.backward([o for o, _ in pairs], [g for _, g in pairs])
@@ -538,7 +548,8 @@ class DataParallelModule(nn.Module):
         self._anchor = None
         try:
             from .arguments import get_args
-            self.preserve_rng = float(getattr(get_args(), "dropout_prob", 0.0)) > 0.0
+            args = get_args()
+            self.preserve_rng = any(float(getattr(args, k, 0.0)) > 0.0 for k in ("dropout_prob", "hidden_dropout", "attention_dropout"))
         except RuntimeError:
             self.preserve_rng = False
 

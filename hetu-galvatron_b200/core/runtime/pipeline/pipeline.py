@@ -24,6 +24,7 @@ from ..arguments import get_args
 from ..backend import get_backend
 from ..comm_groups import CommGroup
 from ..parallel import DataParallelModule, ShardedUnit
+from ..tensor_parallel import random as dropout_random
 from .utils import chunk_batch, chunk_dict
 
 
@@ -346,7 +347,13 @@ class PipelineParallel(nn.Module):
             self.chunk_warning = False
         while len(micro_kwargs) < self.real_chunks:
             micro_kwargs.append(micro_kwargs[-1] if micro_kwargs else {})
+        # (first sample, size) of every microbatch inside the local batch: the dropout context of its forward
+        sizes = [next((t.shape[0] for t in mb if torch.is_tensor(t)), 0) for mb in microbatches[0]]
+        self._mb_span = [(sum(sizes[:i]), sizes[i]) for i in range(len(sizes))]
         return microbatches, micro_kwargs
+
+    def _begin_microbatch(self, i):
+        dropout_random.set_microbatch(*self._mb_span[i])
 
     def update_tensor_shape(self, microbatches, dp_size_input, dp_size, tp_size, sp_size, template_tensor_shape, cp_size=None):
         """Concrete boundary shapes for the regular and the last microbatch (pipeline.py:264-293)."""
@@ -419,6 +426,7 @@ class PipelineParallel(nn.Module):
             if i == n_mb - 1:
                 self.set_last_batch(True)
             cur = [microbatches[0][i], microbatches[1][i]]
+            self._begin_microbatch(i)
             out = self.forward_step(forward_step_function(loss_func, **micro_kwargs[i]), cur, model, None, losses_reduced)
             if profiler is not None and i == n_mb - 1:
                 profiler.profile_memory(iter, "After Forward")
@@ -469,6 +477,7 @@ class PipelineParallel(nn.Module):
             nonlocal fwd_num
             inp = [None] if first else self._recv("prev", shp(fwd_num, in_shape, in_shape_last), in_dt, True)
             cur = [microbatches[0][i], microbatches[1][i]]
+            self._begin_microbatch(i)
             out = self.forward_step(forward_step_function(loss_func, **micro_kwargs[i]), cur, model, inp, losses_reduced)
             fwd_num += 1
             if not last:
@@ -525,6 +534,7 @@ class PipelineParallel(nn.Module):
             shape = in_shape_last if i == n_mb - 1 else in_shape
             inp = [None] if first else self._recv("prev", shape, self.stage_input_tensor_dtype, True)
             cur = [microbatches[0][i], microbatches[1][i]]
+            self._begin_microbatch(i)
             out = self.forward_step(forward_step_function(loss_func, **micro_kwargs[i]), cur, model, inp, losses_reduced)
             if not last:
                 self._send("next", out)

@@ -1,0 +1,140 @@
+"""Dropout randomness of the GPT / BERT families (the role of megatron ``core/tensor_parallel/random.py``).
+
+Hidden-state dropout (embedding output, attention-block output, MLP-block output) draws no state at all: the mask of an element is a
+pure function of (seed, iteration, site, global sample index, global token position, hidden column) -- Philox4x32-10, defined in
+``include/bg_galvatron.h`` -- so TP, Megatron-SP, Ulysses, ZeRO, pipelining and activation recompute all draw the masks a single
+process draws on the global batch, and nothing is stored for backward.  The coordinates come from a per-microbatch *dropout
+context*: the iteration is ``forward_backward``'s ``iter``, the sample base is (data-parallel index x local batch + the offset of the
+microbatch in the contiguous ``chunk`` split, pipeline/utils.py).  ``GalvatronModel.forward_backward`` and the schedules set it;
+``_BiasDropoutAddFn`` copies it into its autograd context and ``_CheckpointFn`` captures it for the recompute.
+
+Site numbering: site = 3 * row + kind, row 0 = the embedding (kind 0), row i + 1 = transformer layer i with kind 1 = attention-block
+output and kind 2 = MLP-block output.
+
+Attention-probability dropout stays inside the attention library call (torch SDPA / flash-attn), whose masks come from torch's
+generator and cannot be made layout-invariant.  It runs under ``RngTracker.fork``: a generator state per (layer, tensor-parallel
+rank, Ulysses rank), seeded like megatron's ``model_parallel_cuda_manual_seed`` (seed + 2718 + ...), so the head slices of
+different ranks are not correlated; the checkpoint recompute replays the tracker state.
+"""
+import collections
+import contextlib
+
+import torch
+
+from ..backend import get_backend
+
+DropoutContext = collections.namedtuple("DropoutContext", "seed iteration sample_base batch")
+
+_CTX = DropoutContext(seed=0, iteration=0, sample_base=0, batch=None)
+_STEP = dict(seed=0, iteration=0, sample_base=0)
+
+SITE_EMBEDDING, SITE_ATTENTION, SITE_MLP = 0, 1, 2
+
+
+def check_probability(p, name="dropout"):
+    """0 <= p < 1, else ValueError (at construction)."""
+    p = float(p)
+    if not 0.0 <= p < 1.0:
+        raise ValueError("%s probability %r must satisfy 0 <= p < 1" % (name, p))
+    return p
+
+
+def site(layer_row, kind):
+    return 3 * int(layer_row) + int(kind)
+
+
+def begin_iteration(seed, iteration, sample_base):
+    """One ``forward_backward`` call: the iteration and the global index of this rank's first sample."""
+    _STEP.update(seed=int(seed), iteration=int(iteration), sample_base=int(sample_base))
+    set_microbatch(0, None)
+
+
+def set_microbatch(offset, size):
+    """Before a microbatch's forward: its first sample is ``offset`` samples into this rank's local batch."""
+    global _CTX
+    _CTX = DropoutContext(_STEP["seed"], _STEP["iteration"], _STEP["sample_base"] + int(offset), None if size is None else int(size))
+
+
+def get_context():
+    return _CTX
+
+
+def set_context(ctx):
+    global _CTX
+    _CTX = ctx
+
+
+class _BiasDropoutAddFn(torch.autograd.Function):
+    """y = residual + keep * scale * (x + bias): one row kernel forward, one backward that regenerates the mask."""
+
+    @staticmethod
+    def forward(ctx, x, bias, residual, p, coords):
+        ctx.p, ctx.coords = p, coords            # (seed, iteration, site, seq_base, sample_base): plain integers, no global state
+        ctx.has_residual, ctx.bias_dtype = residual is not None, None if bias is None else bias.dtype
+        return get_backend().dropout_add_fwd(x, bias, residual, p, *coords)
+
+    @staticmethod
+    def backward(ctx, dy):
+        dx, db = get_backend().dropout_bwd(dy, ctx.p, *ctx.coords, with_bias=ctx.bias_dtype is not None)
+        return dx, (None if db is None else db.to(ctx.bias_dtype)), (dy if ctx.has_residual else None), None, None
+
+
+def bias_dropout_add(x, bias, residual, p, site_id, seq_base=0):
+    """Dropout of an SBH tensor x [s_loc, b_loc, h] (plus bias, plus residual) with the current microbatch's dropout context; the
+    local rows are tokens ``seq_base``.. of the microbatch's samples."""
+    ctx = _CTX
+    if ctx.batch is not None and x.shape[1] != ctx.batch:
+        raise NotImplementedError("dropout: a layer sees %d samples of a %d-sample microbatch (a relocation that re-splits the batch "
+                                  "is not supported with dropout)" % (x.shape[1], ctx.batch))
+    return _BiasDropoutAddFn.apply(x, bias, residual, float(p), (ctx.seed, ctx.iteration, int(site_id), int(seq_base), ctx.sample_base))
+
+
+class RngTracker:
+    """Named generator states swapped into torch's default generator of a device (megatron ``CudaRNGStatesTracker``)."""
+
+    def __init__(self):
+        self.states = {}
+
+    def get_states(self):
+        return {k: v.clone() for k, v in self.states.items()}
+
+    def set_states(self, states):
+        self.states = {k: v.clone() for k, v in states.items()}
+
+    @staticmethod
+    def _get(device):
+        return torch.cuda.get_rng_state(device) if device.type == "cuda" else torch.get_rng_state()
+
+    @staticmethod
+    def _set(state, device):
+        if device.type == "cuda":
+            torch.cuda.set_rng_state(state, device)
+        else:
+            torch.set_rng_state(state)
+
+    @contextlib.contextmanager
+    def fork(self, name, seed, device):
+        key = (name, str(device))
+        if key not in self.states:
+            g = torch.Generator(device=device)
+            g.manual_seed(int(seed))
+            self.states[key] = g.get_state()
+        orig = self._get(device)
+        self._set(self.states[key], device)
+        try:
+            yield
+        finally:
+            self.states[key] = self._get(device)
+            self._set(orig, device)
+
+
+_TRACKER = RngTracker()
+
+
+def get_rng_tracker():
+    return _TRACKER
+
+
+def model_parallel_seed(seed, layer_number, tp_rank, sp_rank):
+    """megatron's ``seed + 2718 + tp_rank``, extended by the Ulysses rank and the layer (so pipeline stages differ as well)."""
+    return int(seed) + 2718 + tp_rank + 64 * sp_rank + 4096 * int(layer_number)

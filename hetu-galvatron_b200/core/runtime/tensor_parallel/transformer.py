@@ -20,6 +20,7 @@ import torch.nn as nn
 
 from ..backend import get_backend
 from .layers import ColumnParallelLinear, RowParallelLinear
+from .random import check_probability, get_rng_tracker, model_parallel_seed
 
 
 class AttnType(enum.Enum):
@@ -120,20 +121,21 @@ class _UlyssesFn(torch.autograd.Function):
 
 class _FlashAttnFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, causal, softmax_scale, key_mask=None):
+    def forward(ctx, q, k, v, causal, softmax_scale, key_mask=None, dropout_p=0.0):
+        drop = {"dropout_p": dropout_p} if dropout_p > 0.0 else {}      # (the backend draws the mask; its backward replays it)
         if key_mask is None:
-            out, lse, rng = get_backend().attention_fwd(q, k, v, causal, softmax_scale)
+            out, lse, rng = get_backend().attention_fwd(q, k, v, causal, softmax_scale, **drop)
         else:
-            out, lse, rng = get_backend().attention_fwd(q, k, v, causal, softmax_scale, key_mask)
+            out, lse, rng = get_backend().attention_fwd(q, k, v, causal, softmax_scale, key_mask, **drop)
         ctx.save_for_backward(q, k, v, out, lse)
-        ctx.causal, ctx.scale, ctx.rng = causal, softmax_scale, rng
+        ctx.causal, ctx.scale, ctx.rng, ctx.drop = causal, softmax_scale, rng, drop
         return out
 
     @staticmethod
     def backward(ctx, dout):
         q, k, v, out, lse = ctx.saved_tensors
-        dq, dk, dv = get_backend().attention_bwd(dout, q, k, v, out, lse, ctx.causal, ctx.scale, ctx.rng)
-        return dq, dk, dv, None, None, None
+        dq, dk, dv = get_backend().attention_bwd(dout, q, k, v, out, lse, ctx.causal, ctx.scale, ctx.rng, **ctx.drop)
+        return dq, dk, dv, None, None, None, None
 
 
 class _LayerNormFn(torch.autograd.Function):
@@ -241,16 +243,17 @@ def _recompute_activations():
         return False
 
 
-def _attention(q, k, v, causal, scale, key_mask=None):
+def _attention(q, k, v, causal, scale, key_mask=None, dropout_p=0.0):
     be = get_backend()
     fn = getattr(be, "attention", None)
+    drop = {"dropout_p": dropout_p} if dropout_p > 0.0 else {}
     if fn is None:
         out = None
     elif key_mask is None:
-        out = fn(q, k, v, causal, scale)                            # differentiable library call (cuDNN SDPA)
+        out = fn(q, k, v, causal, scale, **drop)                    # differentiable library call (cuDNN SDPA)
     else:
-        out = fn(q, k, v, causal, scale, key_mask)
-    return out if out is not None else _FlashAttnFn.apply(q, k, v, causal, scale, key_mask)
+        out = fn(q, k, v, causal, scale, key_mask, **drop)
+    return out if out is not None else _FlashAttnFn.apply(q, k, v, causal, scale, key_mask, dropout_p)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -323,6 +326,27 @@ class ParallelAttention(nn.Module):
                                        input_is_parallel=True, tp_group=tp_group, params_dtype=params_dtype, device=device)
         self.softmax_scale = 1.0 / math.sqrt(self.hn)
         self._identity_rope = {}
+        # dropout on the attention probabilities (GPT / BERT: transformer.py:443-503), in training only, drawn by the attention library
+        # under this layer's model-parallel RNG stream (random.py)
+        self.attention_dropout = check_probability(getattr(config, "attention_dropout", 0.0), "attention_dropout")
+        if self.attention_dropout > 0.0:
+            if self.use_cp:
+                raise NotImplementedError("attention-probability dropout with context parallelism is not supported")
+            try:
+                from ..arguments import get_args
+                seed = int(getattr(get_args(), "seed", 0))
+            except RuntimeError:
+                seed = 0
+            tp_rank = tp_group.rank_in_group() if _size(tp_group) > 1 else 0
+            sp_rank = sp_group.rank_in_group() if self.use_ulysses else 0
+            self._rng_name = ("attention", layer_number, tp_rank, sp_rank)
+            self._rng_seed = model_parallel_seed(seed, layer_number, tp_rank, sp_rank)
+
+    def _core_attention(self, q, k, v, causal, key_mask):
+        if not (self.attention_dropout > 0.0 and self.training):
+            return _attention(q, k, v, causal, self.softmax_scale, key_mask)
+        with get_rng_tracker().fork(self._rng_name, self._rng_seed, q.device):
+            return _attention(q, k, v, causal, self.softmax_scale, key_mask, self.attention_dropout)
 
     def _no_rope(self, seq, device):
         """Families with learned absolute positions (GPT, BERT) run the same split + relayout kernel with cos = 1, sin = 0."""
@@ -349,13 +373,13 @@ class ParallelAttention(nn.Module):
                 rep = self.np_local // self.ng_local
                 k, v = k.repeat_interleave(rep, dim=2), v.repeat_interleave(rep, dim=2)
             q, k, v = _UlyssesFn.apply(self.sp_group, True, q, k, v)       # [b, s, n/p, hn]
-            ctxt = _attention(q, k, v, causal, self.softmax_scale, key_mask)
+            ctxt = self._core_attention(q, k, v, causal, key_mask)
             (ctxt,) = _UlyssesFn.apply(self.sp_group, False, ctxt)         # [b, s/p, n, hn]
         elif self.use_cp:
             assert causal, "context parallelism is implemented for causal self-attention"
             ctxt = _cp_attention(q, k, v, self.cp_group, self.softmax_scale)   # [b, s/c, np, hn]
         else:
-            ctxt = _attention(q, k, v, causal, self.softmax_scale, key_mask)  # [b, s, np, hn]
+            ctxt = self._core_attention(q, k, v, causal, key_mask)          # [b, s, np, hn]
         b, s = ctxt.shape[0], ctxt.shape[1]
         ctxt = ctxt.reshape(b, s, -1).transpose(0, 1).contiguous()          # "b s h d -> s b (h d)"
         return self.dense(ctxt, residual=residual)

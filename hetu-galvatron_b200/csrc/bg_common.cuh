@@ -85,4 +85,24 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
     return v;
 }
 
+// ---- Philox4x32-10 (Salmon et al., SC'11; the generator of curand_philox4x32_x.h) -----------------------------------------
+// Counter-based: the output is a pure function of (counter, key), so a dropout mask needs no state and no stored bits.
+__host__ __device__ __forceinline__ uint32_t philox_mulhi(uint32_t a, uint32_t b) {
+#ifdef __CUDA_ARCH__
+    return __umulhi(a, b);
+#else
+    return (uint32_t)(((uint64_t)a * b) >> 32);
+#endif
+}
+__host__ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+    for (int i = 0; i < 10; ++i) {
+        if (i) { k.x += 0x9E3779B9u; k.y += 0xBB67AE85u; }
+        const uint32_t hi0 = philox_mulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+        const uint32_t hi1 = philox_mulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+        c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    }
+    return c;
+}
+
 }  // namespace bg

@@ -382,6 +382,100 @@ __global__ void __launch_bounds__(kThreads) bias_gelu_kernel(const uint4* __rest
 }
 
 // ---------------------------------------------------------------------------------------------
+// bias + dropout + residual add of the GPT / BERT blocks (the reference's F.dropout sites, GPTModel_tensor_parallel.py:31-59,
+// BertModel_tensor_parallel.py:29-55):  y = residual + keep * scale * (x + bias),  dx = keep * scale * dy.
+// Element (row r, column j) of a local [s_loc, b_loc, h] SBH tensor is token t = seq_base + r / b_loc of sample
+// sample_base + r % b_loc; it is kept iff  Philox4x32-10(ctr = (j / 4, t, sample, iteration), key = (seed, site)).word[j % 4]
+// >= threshold.  The mask depends on global coordinates only -- not on the launch geometry, the rank or the parallel layout --
+// and backward regenerates it (nothing stored).
+// ---------------------------------------------------------------------------------------------
+struct DropoutCoords {
+    long long b_loc, seq_base, sample_base;
+    uint32_t threshold, seed, iteration, site;
+    float scale;
+};
+
+// keep bits of the 8 columns starting at column 8 * c of row r
+__device__ __forceinline__ unsigned dropout_keep8(const DropoutCoords& d, long long r, int c) {
+    const long long tok = r / d.b_loc;
+    const uint32_t t = (uint32_t)(d.seq_base + tok), smp = (uint32_t)(d.sample_base + (r - tok * d.b_loc));
+    const uint2 key = make_uint2(d.seed, d.site);
+    const uint4 a = philox4x32_10(make_uint4(2u * c, t, smp, d.iteration), key);
+    const uint4 b = philox4x32_10(make_uint4(2u * c + 1u, t, smp, d.iteration), key);
+    const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    unsigned bits = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) bits |= (w[i] >= d.threshold ? 1u : 0u) << i;
+    return bits;
+}
+
+// grid = (column blocks, row groups), a thread owns one 8-column vector of every row of its group.  fp32 math in the order
+// (x + bias) * scale, then masked, then + residual, each step rounded once (__fadd_rn / __fmul_rn: no FMA contraction).
+template <bool kBiasF32>
+__global__ void __launch_bounds__(kThreads) dropout_add_fwd_kernel(const uint4* __restrict__ x, const void* __restrict__ bias,
+                                                                   const uint4* __restrict__ residual, uint4* __restrict__ y,
+                                                                   long long rows, int nvec, DropoutCoords d) {
+    const int c = blockIdx.x * kThreads + threadIdx.x;
+    if (c >= nvec) return;
+    float bv[8];
+    if (bias == nullptr) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) bv[i] = 0.f;
+    } else if (kBiasF32) {
+        const float4* bp = reinterpret_cast<const float4*>(bias) + 2 * c;
+        const float4 b0 = __ldg(bp), b1 = __ldg(bp + 1);
+        bv[0] = b0.x; bv[1] = b0.y; bv[2] = b0.z; bv[3] = b0.w; bv[4] = b1.x; bv[5] = b1.y; bv[6] = b1.z; bv[7] = b1.w;
+    } else {
+        unpack8(__ldg(reinterpret_cast<const uint4*>(bias) + c), bv);
+    }
+    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
+        const size_t i = (size_t)r * nvec + c;
+        const uint4 xv = ld16_stream(x + i);
+        uint4 rv = make_uint4(0u, 0u, 0u, 0u);
+        if (residual != nullptr) rv = ld16_stream(residual + i);
+        const unsigned keep = dropout_keep8(d, r, c);
+        float f[8], o[8];
+        unpack8(xv, f);
+        unpack8(rv, o);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const float v = (keep >> k) & 1u ? __fmul_rn(__fadd_rn(f[k], bv[k]), d.scale) : 0.f;
+            o[k] = __fadd_rn(o[k], v);
+        }
+        st16(y + i, pack8(o));
+    }
+}
+
+// dx = keep * scale * dy (bf16);  dbias_partial[blockIdx.y] = the fp32 column sums of keep * scale * dy over the CTA's rows
+__global__ void __launch_bounds__(kThreads) dropout_bwd_kernel(const uint4* __restrict__ dy, uint4* __restrict__ dx,
+                                                               float* __restrict__ dbias_partial, long long rows, int nvec,
+                                                               DropoutCoords d) {
+    const int c = blockIdx.x * kThreads + threadIdx.x;
+    if (c >= nvec) return;
+    float acc[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc[k] = 0.f;
+    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
+        const size_t i = (size_t)r * nvec + c;
+        const uint4 gv = ld16_stream(dy + i);
+        const unsigned keep = dropout_keep8(d, r, c);
+        float g[8];
+        unpack8(gv, g);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            g[k] = (keep >> k) & 1u ? __fmul_rn(g[k], d.scale) : 0.f;
+            acc[k] = __fadd_rn(acc[k], g[k]);
+        }
+        st16(dx + i, pack8(g));
+    }
+    if (dbias_partial != nullptr) {
+        float4* p = reinterpret_cast<float4*>(dbias_partial + ((size_t)blockIdx.y * nvec + c) * 8);
+        p[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+        p[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // swiglu: gate_up = [rows, 2*ffn] (gate = first half, up = second; transformer.py:122-124)
 // ---------------------------------------------------------------------------------------------
 // grid = (column blocks of a row, row groups): no index division; two rows per iteration = four 16-B loads in flight per thread
@@ -792,6 +886,71 @@ extern "C" int bg_bias_gelu(const void* x, const void* bias, const void* dy, voi
     return BG_OK;
 }
 
+extern "C" void bg_philox4x32_10(const uint32_t ctr[4], const uint32_t key[2], uint32_t out[4]) {
+    const uint4 o = philox4x32_10(make_uint4(ctr[0], ctr[1], ctr[2], ctr[3]), make_uint2(key[0], key[1]));
+    out[0] = o.x; out[1] = o.y; out[2] = o.z; out[3] = o.w;
+}
+
+static int dropout_args(long long rows, long long h, long long b_loc, long long seq_base, long long sample_base, double p,
+                        unsigned seed, unsigned iteration, unsigned site, DropoutCoords* d, const char* who) {
+    if (h <= 0 || h % 8) return fail(BG_EINVAL, "%s: hidden %lld must be a positive multiple of 8", who, h);
+    if (h / 8 > (long long)kThreads * 65535) return fail(BG_EUNSUPPORTED, "%s: hidden %lld too wide", who, h);
+    if (rows < 0 || b_loc < 1 || rows % b_loc) return fail(BG_EINVAL, "%s: rows %lld must be a multiple of b_loc %lld", who, rows, b_loc);
+    if (seq_base < 0 || sample_base < 0 || seq_base + rows / b_loc > 0xffffffffLL || sample_base + b_loc > 0xffffffffLL)
+        return fail(BG_EINVAL, "%s: token / sample coordinates must fit 32 bits", who);
+    if (!(p >= 0.0 && p < 1.0)) return fail(BG_EINVAL, "%s: dropout probability %g must be in [0, 1)", who, p);
+    d->b_loc = b_loc; d->seq_base = seq_base; d->sample_base = sample_base;
+    d->threshold = (uint32_t)floor(p * 4294967296.0);
+    d->scale = (float)(1.0 / (1.0 - p));
+    d->seed = seed; d->iteration = iteration; d->site = site;
+    return BG_OK;
+}
+
+// (column blocks, row groups) with about local_ctas CTAs in total
+static dim3 dropout_grid(long long rows, long long nvec, long long want_rows) {
+    const long long cb = (nvec + kThreads - 1) / kThreads;
+    long long gy = want_rows > 0 ? want_rows : g_tun.local_ctas / cb;
+    if (gy < 1) gy = 1;
+    if (want_rows <= 0 && gy > rows) gy = rows > 0 ? rows : 1;
+    if (gy > 65535) gy = 65535;
+    return dim3((unsigned)cb, (unsigned)gy, 1);
+}
+
+extern "C" int bg_dropout_add_fwd(const void* x, const void* bias, int bias_dtype, const void* residual, void* y, long long rows,
+                                  long long h, long long b_loc, long long seq_base, long long sample_base, double p, unsigned seed,
+                                  unsigned iteration, unsigned site, void* stream) {
+    DropoutCoords d;
+    int rc = dropout_args(rows, h, b_loc, seq_base, sample_base, p, seed, iteration, site, &d, "bg_dropout_add_fwd");
+    if (rc) return rc;
+    if (bias != nullptr && bias_dtype != BG_BF16 && bias_dtype != BG_F32) return fail(BG_EUNSUPPORTED, "bg_dropout_add_fwd: bias dtype %d", bias_dtype);
+    if (!BG_ALIGNED16(x) || !BG_ALIGNED16(bias) || !BG_ALIGNED16(residual) || !BG_ALIGNED16(y))
+        return fail(BG_EINVAL, "bg_dropout_add_fwd: 16-B alignment");
+    if (rows == 0) return BG_OK;
+    const dim3 grid = dropout_grid(rows, h / 8, 0);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (bias != nullptr && bias_dtype == BG_F32)
+        dropout_add_fwd_kernel<true><<<grid, kThreads, 0, st>>>((const uint4*)x, bias, (const uint4*)residual, (uint4*)y, rows, (int)(h / 8), d);
+    else
+        dropout_add_fwd_kernel<false><<<grid, kThreads, 0, st>>>((const uint4*)x, bias, (const uint4*)residual, (uint4*)y, rows, (int)(h / 8), d);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_dropout_bwd(const void* dy, void* dx, float* dbias_partial, int n_partial, long long rows, long long h, long long b_loc,
+                              long long seq_base, long long sample_base, double p, unsigned seed, unsigned iteration, unsigned site,
+                              void* stream) {
+    DropoutCoords d;
+    int rc = dropout_args(rows, h, b_loc, seq_base, sample_base, p, seed, iteration, site, &d, "bg_dropout_bwd");
+    if (rc) return rc;
+    if (n_partial < 1 || n_partial > 65535) return fail(BG_EINVAL, "bg_dropout_bwd: n_partial %d must be in [1, 65535]", n_partial);
+    if (!BG_ALIGNED16(dy) || !BG_ALIGNED16(dx) || !BG_ALIGNED16(dbias_partial)) return fail(BG_EINVAL, "bg_dropout_bwd: 16-B alignment");
+    // (rows == 0 still launches: every one of the n_partial CTAs writes its partial row, zeros if it visits no row)
+    dropout_bwd_kernel<<<dropout_grid(rows, h / 8, n_partial), kThreads, 0, (cudaStream_t)stream>>>((const uint4*)dy, (uint4*)dx, dbias_partial,
+                                                                                                   rows, (int)(h / 8), d);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
 // loads every kernel of this file up front (see bg_preload_coll in bg_coll.cu)
 int bg_preload_ops() {
 #define K(f) reinterpret_cast<const void*>(&f)
@@ -800,7 +959,8 @@ int bg_preload_ops() {
                              K((bias_gelu_kernel<true, false>)), K((bias_gelu_kernel<false, false>)), K((bias_gelu_kernel<true, true>)),
                              K((bias_gelu_kernel<false, true>)), K(swiglu_fwd_kernel), K(swiglu_bwd_kernel), K(qkv_rope_kernel),
                              K(ce_rowmax_kernel<true>), K(ce_rowmax_kernel<false>), K(ce_sumexp_kernel<true>), K(ce_sumexp_kernel<false>),
-                             K(ce_bwd_kernel<true>), K(ce_bwd_kernel<false>)};
+                             K(ce_bwd_kernel<true>), K(ce_bwd_kernel<false>), K(dropout_add_fwd_kernel<true>),
+                             K(dropout_add_fwd_kernel<false>), K(dropout_bwd_kernel)};
 #undef K
     for (const void* k : kernels) {
         cudaFuncAttributes attr;

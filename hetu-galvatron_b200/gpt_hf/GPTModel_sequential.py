@@ -8,10 +8,22 @@ from ..core.runtime.pipeline import PipeSequential
 from ..core.runtime.tensor_parallel import (VocabUtility, gather_from_tensor_model_parallel_region_group,
                                             linear_with_grad_accumulation_and_async_allreduce,
                                             scatter_to_sequence_parallel_region_group, vocab_parallel_cross_entropy)
+from ..core.runtime.tensor_parallel.random import SITE_EMBEDDING, bias_dropout_add, check_probability, site
 
 
 def _size(g):
     return 1 if g is None else g.size
+
+
+def _embedding_dropout(module, hidden_states):
+    """Embedding dropout (hidden_dropout) on the SBH slice this rank holds after the vocab_sp slice and the Megatron-SP scatter, at
+    global token positions."""
+    if not (module.dropout_p > 0.0 and module.training):
+        return hidden_states
+    seq_base = module.seq_start_index if module.vocab_sp else 0
+    if module.sequence_parallel and _size(module.tp_group) > 1:
+        seq_base += module.tp_group.rank_in_group() * hidden_states.shape[0]
+    return bias_dropout_add(hidden_states, None, None, module.dropout_p, site(0, SITE_EMBEDDING), seq_base)
 
 
 def _seq_slice(args, sp_group):
@@ -48,6 +60,7 @@ class GPTEmbeddings_(nn.Module):
         self.vocab_sp = args.vocab_sp
         if self.vocab_sp:
             self.seq_start_index, self.seq_end_index = _seq_slice(args, self.sp_group)
+        self.dropout_p = check_probability(getattr(args, "hidden_dropout", 0.0), "hidden_dropout")     # :55
 
     def forward(self, tokens, position_ids=None, attention_mask=None, labels=None):
         if position_ids is None:
@@ -59,7 +72,7 @@ class GPTEmbeddings_(nn.Module):
         hidden_states = hidden_states.transpose(0, 1).contiguous()           # [b, s, h] -> [s, b, h]
         if self.sequence_parallel:
             hidden_states = scatter_to_sequence_parallel_region_group(hidden_states, self.tp_group)
-        return hidden_states                                                  # (dropout 0 on the random-data path, config_utils.py:98-99)
+        return _embedding_dropout(self, hidden_states)
 
 
 class GPTLayers_(nn.Module):

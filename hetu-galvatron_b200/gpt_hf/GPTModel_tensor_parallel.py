@@ -7,6 +7,7 @@ from torch import nn
 from ..core.runtime.arguments import get_args
 from ..core.runtime.tensor_parallel import (AttnMaskType, AttnType, ColumnParallelLinear, LayerNorm, ParallelAttention, ParallelMLP,
                                             VocabParallelEmbedding)
+from ..core.runtime.tensor_parallel.random import SITE_ATTENTION, SITE_MLP, bias_dropout_add, check_probability, site
 
 
 def core_transformer_config_from_args(args):
@@ -16,11 +17,23 @@ def core_transformer_config_from_args(args):
         hidden_size=args.hidden_size, ffn_hidden_size=args.ffn_hidden_size, num_attention_heads=args.num_attention_heads,
         num_query_groups=args.num_attention_heads, kv_channels=args.hidden_size // args.num_attention_heads,
         layernorm_epsilon=args.norm_epsilon, init_method_std=args.init_method_std, sequence_parallel=args.sequence_parallel,
-        gated_linear_unit=False, add_bias_linear=True, gelu_tanh=True)
+        gated_linear_unit=False, add_bias_linear=True, gelu_tanh=True,
+        hidden_dropout=check_probability(getattr(args, "hidden_dropout", 0.0), "hidden_dropout"),
+        attention_dropout=check_probability(getattr(args, "attention_dropout", 0.0), "attention_dropout"))
 
 
 def _megatron_sp(args, tp_group):
     return bool(args.sequence_parallel) and tp_group is not None and tp_group.size > 1
+
+
+def _seq_rank(args, tp_group, sp_group):
+    """Index of the sequence slice a block's [s/p, b, h] activations hold: the Ulysses rank, the Megatron-SP (tensor-parallel) rank,
+    or 0 when the block sees the whole sequence.  Dropout masks are drawn at global token positions seq_rank * s/p + local row."""
+    if sp_group is not None and sp_group.size > 1:
+        return sp_group.rank_in_group()
+    if _megatron_sp(args, tp_group):
+        return tp_group.rank_in_group()
+    return 0
 
 
 class GPTAttention_tp(nn.Module):
@@ -35,17 +48,24 @@ class GPTAttention_tp(nn.Module):
                                            tp_group=self.tp_group, sp_group=self.sp_group, use_ulysses=self.use_ulysses, device="meta")
         self.LayerNorm = LayerNorm(config.hidden_size, eps=config.layer_norm_epsilon, device="meta",
                                    sequence_parallel=_megatron_sp(args, tp_group))
+        # the reference drops the attention-block output with attention_dropout, not hidden_dropout (:31-39): kept on purpose
+        self.dropout_p, self.site = mconf.attention_dropout, site(layer_number + 1, SITE_ATTENTION)
+        self.seq_rank = _seq_rank(args, tp_group, sp_group)
 
     def forward(self, hidden_states, attention_mask):
         residual = hidden_states
         hidden_states = self.LayerNorm(hidden_states)
+        if self.dropout_p > 0.0 and self.training:
+            # after the projection's reduction (all-reduce / reduce-scatter): one row kernel for bias + dropout + residual
+            out, bias = self.attention(hidden_states, None)
+            return bias_dropout_add(out, bias, residual, self.dropout_p, self.site, self.seq_rank * out.shape[0])
         # causal: the mask is implied (flash path, :36-41); the residual add (:42) rides in the projection GEMM's epilogue
         hidden_states, bias = self.attention(hidden_states, None, residual=residual)
         return hidden_states if bias is None else hidden_states + bias
 
 
 class GPTMLP_tp(nn.Module):
-    def __init__(self, config, tp_group=None):
+    def __init__(self, config, tp_group=None, layer_number=0, sp_group=None):
         super().__init__()
         args = get_args()
         mconf = core_transformer_config_from_args(args)
@@ -53,10 +73,15 @@ class GPTMLP_tp(nn.Module):
         self.mlp = ParallelMLP(mconf, tp_group=self.tp_group, device="meta")
         self.LayerNorm = LayerNorm(config.hidden_size, eps=config.layer_norm_epsilon, device="meta",
                                    sequence_parallel=_megatron_sp(args, tp_group))
+        self.dropout_p, self.site = mconf.hidden_dropout, site(layer_number + 1, SITE_MLP)        # :51-59
+        self.seq_rank = _seq_rank(args, tp_group, sp_group)
 
     def forward(self, hidden_states):
         residual = hidden_states
         hidden_states = self.LayerNorm(hidden_states)
+        if self.dropout_p > 0.0 and self.training:
+            out, bias = self.mlp(hidden_states)
+            return bias_dropout_add(out, bias, residual, self.dropout_p, self.site, self.seq_rank * out.shape[0])
         hidden_states, bias = self.mlp(hidden_states, residual=residual)
         return hidden_states if bias is None else hidden_states + bias
 
@@ -65,7 +90,7 @@ class GPTLayer_tp(nn.Module):
     def __init__(self, config, layer_number, tp_group=None, sp_group=None):
         super().__init__()
         self.attention = GPTAttention_tp(config, layer_number, tp_group, sp_group)
-        self.mlp = GPTMLP_tp(config, tp_group)
+        self.mlp = GPTMLP_tp(config, tp_group, layer_number, sp_group)
         self.idx = layer_number
 
     def forward(self, hidden_states, attention_mask=None):

@@ -20,6 +20,9 @@ def config_from_meta(model_type):
         hidden_size=h, num_hidden_layers=p["n_layer"], num_attention_heads=p["n_head"], num_key_value_heads=p["n_head"],
         intermediate_size=p.get("n_inner") or 4 * h, vocab_size=p["vocab_size"], max_position_embeddings=p["n_positions"],
         layer_norm_epsilon=p.get("layer_norm_epsilon", 1e-5), attention_dropout=0.0,
+        # GPT2Config's dropouts (0.1 each in HF; 0 in the shipped specs here, see arguments.hidden_dropout)
+        resid_pdrop=float(p.get("resid_pdrop", 0.0)), embd_pdrop=float(p.get("embd_pdrop", p.get("resid_pdrop", 0.0))),
+        attn_pdrop=float(p.get("attn_pdrop", 0.0)),
         model_name=model_type if isinstance(model_type, str) else "custom")
 
 
@@ -38,4 +41,7 @@ def set_model_config(config, args, overwrite_args=True):
         args.vocab_size = config.vocab_size
         mult = getattr(args, "make_vocab_size_divisible_by", 128) * max(1, getattr(args, "vocab_tp", 1))
         args.padded_vocab_size = (config.vocab_size + mult - 1) // mult * mult   # megatron _vocab_size_with_padding
+        # config_utils.py:74-76 (overwrite_megatron_args): one hidden dropout for the embedding and the residual branches
+        assert abs(config.resid_pdrop - config.embd_pdrop) <= 1e-3, "resid_pdrop should be equal to embd_pdrop"
+        args.hidden_dropout, args.attention_dropout = config.resid_pdrop, config.attn_pdrop
     return config

@@ -167,6 +167,25 @@ int bg_layernorm_bwd(const void* dy, const void* x, const void* w, const float* 
 /* bias + GeLU of the GPT / BERT MLP (transformer.py:150-160 bias_gelu_impl): out = gelu(x + bias) when dy == NULL, else
  * out = dy * gelu'(x + bias).  tanh_form 1 = Megatron's fused / HF gelu_new, 0 = exact erf.  bias may be NULL. */
 int bg_bias_gelu(const void* x, const void* bias, const void* dy, void* out, long long rows, long long cols, int tanh_form, void* stream);
+/* bias + dropout + residual add of the GPT / BERT blocks, replacing the reference's F.dropout(x + bias) + residual at
+ * GPTModel_tensor_parallel.py:31-39,51-59, BertModel_tensor_parallel.py:29-36,48-55 and the embedding dropouts
+ * (GPTModel_sequential.py:55, BertModel_sequential.py:100-102):  y = residual + keep * scale * (x + bias), fp32 math, one rounding
+ * per step.  x, residual, y: bf16 [rows][h] rows of a local [s_loc][b_loc][h] tensor; row r is token seq_base + r / b_loc of
+ * sample sample_base + r % b_loc.  Element (token t, sample b, column j) is kept iff
+ *     Philox4x32-10(counter = {j / 4, t, b, iteration}, key = {seed, site}).word[j % 4] >= floor(p * 2^32)
+ * and kept values are scaled by (float)(1 / (1 - p)).  The mask depends on these global coordinates only, so every parallel
+ * layout draws the same mask.  bias (bf16 or fp32 [h]) and residual may be NULL.  h % 8 == 0, 0 <= p < 1. */
+int bg_dropout_add_fwd(const void* x, const void* bias, int bias_dtype, const void* residual, void* y, long long rows, long long h,
+                       long long b_loc, long long seq_base, long long sample_base, double p, unsigned seed, unsigned iteration,
+                       unsigned site, void* stream);
+/* its backward (the residual's gradient is dy itself): dx = bf16(keep * scale * dy) with the mask regenerated from the same
+ * arguments; dbias_partial (may be NULL) = [n_partial][h] fp32 per-CTA column sums of keep * scale * dy (the caller adds them). */
+int bg_dropout_bwd(const void* dy, void* dx, float* dbias_partial, int n_partial, long long rows, long long h, long long b_loc,
+                   long long seq_base, long long sample_base, double p, unsigned seed, unsigned iteration, unsigned site,
+                   void* stream);
+/* host-only: one Philox4x32-10 block (the generator of curand_philox4x32_x.h), so the mask definition can be checked without a
+ * GPU.  No CUDA call. */
+void bg_philox4x32_10(const uint32_t ctr[4], const uint32_t key[2], uint32_t out[4]);
 int bg_swiglu_fwd(const void* gate_up, void* y, long long rows, long long ffn, void* stream);
 int bg_swiglu_bwd(const void* dy, const void* gate_up, void* dgate_up, long long rows, long long ffn, void* stream);
 /* fused QKV split + RoPE + [s,b,ng,(r+2)*hn] -> q [b,s,ng*r,hn], k/v [b,s,ng,hn] relayout; backward=1 is the exact

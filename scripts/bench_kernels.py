@@ -1,5 +1,5 @@
 """Micro-benchmarks of the C-ABI kernels on one GPU (CUDA events, warm-up, L2-exceeding inputs).
-Usage: python scripts/bench_kernels.py [gemm] [cast] [ops] [attn]  -> JSON lines on stdout."""
+Usage: python scripts/bench_kernels.py [gemm] [cast] [ops] [attn] [dropout]  -> JSON lines on stdout."""
 import json
 import os
 import sys
@@ -211,6 +211,78 @@ def attn():
         for name, o in results.items():
             print(json.dumps({"bench": "attention_parity", "impl": name,
                               "max_abs_diff_vs_flash_attn2": float((o.float() - results["flash_attn2"].float()).abs().max())}), flush=True)
+
+
+def dropout():
+    """The bias + dropout + residual row kernels at the GPT-3 6.7B leg shape (h 4096, seq 2048) and the BERT-large leg shape
+    (h 1024, seq 8192), microbatch 4, against torch's eager ``F.dropout(x + b) + r`` and its backward (``native_dropout_backward``
+    on the stored mask + the bias-gradient column sum), interleaved round by round on two input sets of > 50 MB each.
+    Algorithmic bytes: forward reads x and the residual and writes y (6 B / element; torch also writes and reads a 1-B mask and
+    the x + b temporary), backward reads dy and writes dx (4 B / element; ours regenerates the mask).  Also probes which SDPA
+    backends accept dropout on the attention probabilities at those shapes."""
+    import subprocess
+    import torch.nn.functional as F
+    from torch.nn.attention import SDPBackend, sdpa_kernel
+    from hetu_galvatron_b200.core.runtime.backend import CudaBackend
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    print(json.dumps({"nvidia_smi": q.stdout.strip()}), flush=True)
+    be = CudaBackend(arena_bytes=1 << 24)
+    p, rounds = 0.1, 5
+    for name, s, h in (("gpt3_6.7b", 2048, 4096), ("bert_large", 8192, 1024)):
+        b = 4
+        sets = [tuple(torch.randn(s, b, h, device="cuda").to(BF) for _ in range(3)) + (torch.randn(h, device="cuda").to(BF),) for _ in range(2)]
+        masks = [torch.rand(s, b, h, device="cuda") >= p for _ in range(2)]
+        n = s * b * h
+        iters = 20
+
+        arms = {
+            "ours_fwd": lambda st, m: be.dropout_add_fwd(st[0], st[3], st[1], p, 1234, 7, 5, 0, 0),
+            "torch_fwd": lambda st, m: F.dropout(st[0] + st[3], p) + st[1],
+            "ours_bwd": lambda st, m: be.dropout_bwd(st[2], p, 1234, 7, 5, 0, 0, with_bias=True),
+            "torch_bwd": lambda st, m: (lambda dx: (dx, dx.sum((0, 1))))(torch.ops.aten.native_dropout_backward(st[2], m, 1.0 / (1.0 - p))),
+        }
+
+        def window(fn):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for i in range(iters):
+                fn(sets[i % 2], masks[i % 2])
+            e1.record()
+            torch.cuda.synchronize()
+            return e0.elapsed_time(e1) / iters
+
+        times = {k: [] for k in arms}
+        for fn in arms.values():
+            window(fn)
+        for _ in range(rounds):
+            for k, fn in arms.items():
+                times[k].append(window(fn))
+        rec = {"bench": "dropout", "shape": name, "s": s, "b": b, "h": h, "p": p}
+        for k, ts in times.items():
+            t = sorted(ts)[rounds // 2]
+            nbytes = (6 if k.endswith("fwd") else 4) * n
+            rec[k + "_ms"] = round(t, 4)
+            rec[k + "_GBps_algorithmic"] = round(nbytes / t / 1e6, 1)
+            rec[k + "_pct_of_3350GBps"] = round(100 * nbytes / t / 1e6 / 3350, 1)
+            rec[k + "_spread_pct"] = round(100 * (max(ts) - min(ts)) / t, 1)
+        print(json.dumps(rec), flush=True)
+        # which SDPA kernels take dropout_p at this shape (32 heads of 128 for GPT, 16 of 64 for BERT; causal for GPT)
+        heads, hd = (32, 128) if name.startswith("gpt") else (16, 64)
+        qkv = [torch.randn(1, heads, min(s, 4096), hd, device="cuda", dtype=BF, requires_grad=True) for _ in range(3)]
+        ok = {}
+        for bk in (SDPBackend.CUDNN_ATTENTION, SDPBackend.FLASH_ATTENTION, SDPBackend.EFFICIENT_ATTENTION):
+            try:
+                with sdpa_kernel([bk]):
+                    o = F.scaled_dot_product_attention(*qkv, dropout_p=0.1, is_causal=name.startswith("gpt"))
+                    o.sum().backward()
+                torch.cuda.synchronize()
+                ok[bk.name] = True
+            except RuntimeError as e:
+                ok[bk.name] = "refused: " + str(e).splitlines()[0][:120]
+        print(json.dumps({"bench": "sdpa_dropout_backends", "shape": name, "accepts_dropout": ok}), flush=True)
+        del sets, masks
+        torch.cuda.empty_cache()
+    be.close()
 
 
 if __name__ == "__main__":
