@@ -20,7 +20,9 @@ LIB_PATH = os.path.join(_HERE, "csrc", "libbg_galvatron.so")
 BF16, F32 = 0, 1
 SUM, MAX = 0, 1
 MAX_PEERS = 8
-LANE_UNSHARD, LANE_REDUCE, LANE_ACT, LANE_MISC, LANE_PUSH = 0, 1, 2, 3, 4
+# LANE_RING: the context-parallel ring's hop flags (bg_cp_ring_*), nothing else
+LANE_UNSHARD, LANE_REDUCE, LANE_ACT, LANE_MISC, LANE_PUSH, LANE_RING = 0, 1, 2, 3, 4, 5
+RING_KV, RING_ACC = 0, 1
 
 _c = ctypes
 _vp, _sz, _i, _ll, _f = _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_longlong, _c.c_float
@@ -71,6 +73,11 @@ SIGNATURES = {
     "bg_p2p_send": (_i, [_vp, _i, _sz, _vp, _sz, _i, _vp]),
     "bg_p2p_wait": (_i, [_vp, _i, _i, _vp]),
     "bg_p2p_release": (_i, [_vp, _i, _i, _vp]),
+    "bg_cp_ring_push": (_i, [_vp, _i, _i, _i, _vp, _vp, _sz, _c.POINTER(_sz), _vp]),
+    "bg_cp_ring_acc_push": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _c.POINTER(_sz), _vp]),
+    "bg_cp_ring_wait": (_i, [_vp, _i, _i, _i, _sz, _vp]),
+    "bg_cp_ring_release": (_i, [_vp, _i, _i, _i, _sz, _vp]),
+    "bg_lse_merge": (_i, [_vp, _vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _i, _vp]),
     "bg_cast": (_i, [_vp, _i, _vp, _i, _sz, _f, _i, _vp]),
     "bg_rmsnorm_fwd": (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _f, _vp]),
     "bg_rmsnorm_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _ll, _ll, _i, _vp]),
@@ -587,6 +594,25 @@ class BgComm:
     def p2p_release(self, peer_rank, flag_id, stream=None):
         check(lib().bg_p2p_release(self._ctx, int(peer_rank), int(flag_id), _stream_ptr(stream)))
 
+    # ---- ring context parallelism: one hop to the next member of ``group`` (include/bg_galvatron.h, C15) ----
+    def cp_ring_push(self, group, slot, parity, wait_free, k, v, stream=None):
+        """k, v (bf16, same numel) -> the next member's ``slot`` (SymBuffer view offsets of the parity's [k | v] slot)."""
+        check(lib().bg_cp_ring_push(self._ctx, self.group_id(group), int(parity), 1 if wait_free else 0, _ptr(k), _ptr(v), k.numel(),
+                                    slot, _stream_ptr(stream)))
+
+    def cp_ring_acc_push(self, group, slot, parity, wait_free, acc_in, dk, dv, batch, rows, row_elems, c_row0, c_rows, stream=None):
+        """next member's fp32 [dK | dV] slot = acc_in (or 0) + the bf16 contribution rows c_row0 .. c_row0 + c_rows - 1."""
+        check(lib().bg_cp_ring_acc_push(self._ctx, self.group_id(group), int(parity), 1 if wait_free else 0,
+                                        _ptr(acc_in) if acc_in is not None else None, _ptr(dk) if dk is not None else None,
+                                        _ptr(dv) if dv is not None else None, int(batch), int(rows), int(row_elems), int(c_row0),
+                                        int(c_rows), slot, _stream_ptr(stream)))
+
+    def cp_ring_wait(self, group, kind, parity, elems, stream=None):
+        check(lib().bg_cp_ring_wait(self._ctx, self.group_id(group), int(kind), int(parity), int(elems), _stream_ptr(stream)))
+
+    def cp_ring_release(self, group, kind, parity, elems, stream=None):
+        check(lib().bg_cp_ring_release(self._ctx, self.group_id(group), int(kind), int(parity), int(elems), _stream_ptr(stream)))
+
     def error_flag(self):
         out = _i()
         check(lib().bg_ctx_error_flag(self._ctx, ctypes.byref(out)))
@@ -604,6 +630,17 @@ class BgComm:
 def cast(src, dst, scale=1.0, accumulate=False, stream=None):
     check(lib().bg_cast(_ptr(src), dtype_code(src.dtype), _ptr(dst), dtype_code(dst.dtype), src.numel(), float(scale),
                         1 if accumulate else 0, _stream_ptr(stream)))
+
+
+def lse_merge(blk_out, blk_lse, acc_out, acc_lse, final_out=None, row_off=0, init=False, stream=None):
+    """Merge one attention block (out [b, sq_blk, n, d] bf16, lse [b, n, sq_blk] fp32) into the running fp32 (acc_out [b, s, n, d],
+    acc_lse [b, n, s]) at query rows row_off..; ``final_out`` (bf16 [b, s, n, d]): also write the merged output there."""
+    b, s, n, d = acc_out.shape
+    for t in (blk_out, blk_lse, acc_out, acc_lse) + ((final_out,) if final_out is not None else ()):
+        if not t.is_contiguous():
+            raise BgError("lse_merge operands must be contiguous")
+    check(lib().bg_lse_merge(_ptr(blk_out), _ptr(blk_lse), _ptr(acc_out), _ptr(acc_lse), _ptr(final_out) if final_out is not None else None,
+                             b, s, blk_out.shape[1], n, d, int(row_off), 1 if init else 0, _stream_ptr(stream)))
 
 
 def gemm_bf16_add(a, b, c, addend, m, n, k, layout, stream=None):

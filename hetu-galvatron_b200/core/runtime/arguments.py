@@ -72,6 +72,8 @@ DEFAULTS = dict(
                                          # elementwise pass in backward -- 352 MiB less per 8B layer at seq 8192
     untie_embeddings_and_output_weights=True,   # megatron's flag; the tied path (C14, grad_reduce.py:98-131) is not built
     zero3_pool_slots=4,                  # rotating peer-visible buffers the zero3 layers of one group gather into (0 = one per layer)
+    cp_comm="allgather",                 # context parallelism's K/V exchange: "allgather" (whole-sequence K/V per layer, one gather) or
+                                         # "ring" (only the local s/c rows kept; blocks travel between neighbours, c-1 hops)
 )
 
 

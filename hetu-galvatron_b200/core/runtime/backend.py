@@ -155,6 +155,35 @@ class CudaBackend:
             self._staging[key] = buf
         return self._staging[key]
 
+    def reserve_cp_ring(self, group, elems):
+        """Receive slots of the context-parallel ring for ``group`` (``cp_comm="ring"``): a region of their own, sized for a local
+        K block of ``elems`` elements -- per step parity one [K | V] bf16 slot and one [dK | dV] fp32 slot, 24 B per element.  Before
+        ``exchange()``, identically on every member."""
+        if group is None or group.size == 1:
+            return
+        rings = self.__dict__.setdefault("_cp_ring_bufs", {})
+        key = tuple(group.ranks)
+        elems = (int(elems) + 7) // 8 * 8
+        cur = rings.get(key)
+        if cur is None or cur[1] < elems:
+            if cur is not None and cur[0].offsets is not None:
+                raise self.bg.BgError("cp ring slots of group %s are already exchanged" % (key,))
+            rings[key] = (self.comm.sym_alloc(group, _CpRing.slot_bytes(elems)), elems)
+
+    def cp_ring(self, group):
+        """The ring transport of ``group`` (one per group: its flags' first-use state is shared by every layer on the group)."""
+        key = tuple(group.ranks)
+        rings = self.__dict__.setdefault("_cp_rings", {})
+        if key not in rings:
+            buf = self.__dict__.get("_cp_ring_bufs", {}).get(key)
+            if buf is None:
+                raise self.bg.BgError("no cp ring slots reserved for group %s (models built with cp_comm='ring' reserve them)" % (key,))
+            rings[key] = _CpRing(self.comm, group, buf[0], buf[1], comm_stream=self.comm_stream, counts=self.n_fused)
+        return rings[key]
+
+    def lse_merge(self, blk_out, blk_lse, acc_out, acc_lse, final_out=None, row_off=0, init=False):
+        self.bg.lse_merge(blk_out.contiguous(), blk_lse.contiguous(), acc_out, acc_lse, final_out, row_off, init)
+
     def staging(self, group, nbytes, byte_offset=0):
         buf = self._staging.get(tuple(group.ranks))
         if buf is None or buf.data_bytes < nbytes + byte_offset:
@@ -755,6 +784,107 @@ class CudaBackend:
 
     def launch_count(self):
         return self.bg.launch_count()
+
+
+class _CpRing:
+    """Peer-HBM transport of the context-parallel ring (include/bg_galvatron.h, C15): step i of a schedule holds the K/V block that
+    arrived in slot parity i % 2 and pushes it on into the next member's slot (i + 1) % 2.  The K/V push runs on ``comm_stream``
+    (when given), ordered after the work already queued, so it overlaps the step's attention; the accumulate-and-forward push
+    depends on the step's gradients and runs in stream order.  A push into a parity waits for the receiver's release of it, except
+    on the slot's very first use."""
+
+    @staticmethod
+    def slot_bytes(elems):
+        return 2 * (2 * elems * 2 + 2 * elems * 4)
+
+    def __init__(self, comm, group, buf, capacity, comm_stream=None, counts=None):
+        from ... import _bg
+        self.bg, self.comm, self.group, self.buf, self.capacity = _bg, comm, group, buf, int(capacity)
+        self.size, self.rank = group.size, group.rank_in_group(comm.rank)
+        self.comm_stream, self.counts = comm_stream, counts
+        self._used = set()             # (kind, parity) pushed into at least once
+        self._pushed = {}              # parity of the slot a K/V push read -> its completion event (comm_stream)
+        self.shape = None
+
+    def _kv_off(self, parity):
+        return parity * 4 * self.capacity
+
+    def _acc_off(self, parity):
+        return 8 * self.capacity + parity * 8 * self.capacity
+
+    def _first(self, kind, parity):
+        first = (kind, parity) not in self._used
+        self._used.add((kind, parity))
+        return first
+
+    def _count(self):
+        if self.counts is not None:
+            self.counts["cp_ring"] = self.counts.get("cp_ring", 0) + 1
+
+    def _check(self, t):
+        if t.numel() > self.capacity:
+            raise self.bg.BgError("cp ring block of %d elements > the %d reserved" % (t.numel(), self.capacity))
+
+    def send_kv(self, step, k, v):
+        """push this step's K/V block to the next member, for its step + 1"""
+        self._check(k)
+        self.shape = tuple(k.shape)
+        parity = (step + 1) % 2
+        wait_free = not self._first(0, parity)
+        slot = self.buf.sub(self._kv_off(parity))
+        if self.comm_stream is None:
+            self.comm.cp_ring_push(self.group, slot, parity, wait_free, k, v)
+        else:
+            cur = torch.cuda.current_stream()
+            self.comm_stream.wait_stream(cur)
+            self.comm.cp_ring_push(self.group, slot, parity, wait_free, k, v, stream=self.comm_stream)
+            if step > 0:               # (step 0 pushes the rank's own block, not a slot)
+                ev = torch.cuda.Event()
+                ev.record(self.comm_stream)
+                self._pushed[step % 2] = ev
+            k.record_stream(self.comm_stream)
+            v.record_stream(self.comm_stream)
+        self._count()
+
+    def recv_kv(self, step):
+        """(k, v) of this step: views of the receive slot, valid until ``release_kv(step)``"""
+        n = 1
+        for d in self.shape:
+            n *= d
+        self.comm.cp_ring_wait(self.group, self.bg.RING_KV, step % 2, n)
+        kv = self.buf.u8[self._kv_off(step % 2): self._kv_off(step % 2) + 4 * n].view(torch.bfloat16)
+        return kv[:n].view(self.shape), kv[n:].view(self.shape)
+
+    def release_kv(self, step):
+        ev = self._pushed.pop(step % 2, None)
+        if ev is not None:             # the push that forwarded this slot has read it
+            torch.cuda.current_stream().wait_event(ev)
+        n = 1
+        for d in self.shape:
+            n *= d
+        self.comm.cp_ring_release(self.group, self.bg.RING_KV, step % 2, n)
+
+    def send_acc(self, step, acc_in, dk, dv, c_row0, c_rows):
+        """next member's [dK | dV] = acc_in (None at step 0) + this step's dk, dv (rows c_row0 .. of the block)"""
+        b, s, ng, d = self.shape
+        parity = (step + 1) % 2
+        self.comm.cp_ring_acc_push(self.group, self.buf.sub(self._acc_off(parity)), parity, not self._first(1, parity), acc_in,
+                                   dk.contiguous(), dv.contiguous(), b, s, ng * d, c_row0, c_rows)
+        self._count()
+
+    def recv_acc(self, step):
+        """the fp32 [dK | dV] accumulators that arrived for this step (step = size: the finished sums, back at their owner)"""
+        n = 1
+        for d in self.shape:
+            n *= d
+        self.comm.cp_ring_wait(self.group, self.bg.RING_ACC, step % 2, n)
+        return self.buf.u8[self._acc_off(step % 2): self._acc_off(step % 2) + 8 * n].view(torch.float32)
+
+    def release_acc(self, step):
+        n = 1
+        for d in self.shape:
+            n *= d
+        self.comm.cp_ring_release(self.group, self.bg.RING_ACC, step % 2, n)
 
 
 class _Timed:

@@ -19,6 +19,7 @@ from .hybrid_parallel_config import (check_hp_config, get_chunks, hp_config_whol
                                      mixed_precision_dtype)
 from .parallel import finalize_pools, wrap_modules_relocation
 from .tensor_parallel import random as dropout_random
+from .tensor_parallel.transformer import ParallelAttention, cp_comm_mode
 
 
 class GalvatronModel(nn.Module):
@@ -109,6 +110,7 @@ def construct_hybrid_parallel_model_api(model, model_config, training_args, hybr
     if wrap_checkpoint_block_name is None:
         wrap_checkpoint_block_name = wrap_block_name
     config, args, hp_configs = model_config, training_args, hybrid_parallel_configs
+    cp_comm_mode()          # an unknown cp_comm raises ValueError here, before any group or buffer exists
     be = get_backend()
 
     info = model_info(config, args)
@@ -218,6 +220,16 @@ def _reserve_activation_staging(be, args, info, hp_whole, hp_model, tp_groups, s
         for lst in (tp_groups, sp_groups, split_sep_groups, allgather_sep_groups, fused_ag_groups, fused_sp_groups, cp_groups or ()):
             if lst:
                 reserve(lst[i])
+    # cp_comm="ring": receive slots of their own per cp group, for the largest local K block (microbatch x s/c x kv heads x head dim)
+    # of this stage's context-parallel layers -- 2 x (K + V) bf16 + 2 x (dK + dV) fp32, more than the staging estimate above
+    ring_elems = {}
+    for m in hp_model.modules():
+        if isinstance(m, ParallelAttention) and m.use_cp and m.cp_comm == "ring" and m.cp_group is not None and m.cp_group.size > 1:
+            key = tuple(m.cp_group.ranks)
+            elems = max_mbs * (seq // m.cp_group.size) * m.ng_local * m.hn
+            ring_elems[key] = (m.cp_group, max(elems, ring_elems.get(key, (None, 0))[1]))
+    for group, elems in ring_elems.values():
+        be.reserve_cp_ring(group, elems)
     # the whole job as one group (gradient-norm all-reduce of clip_grad_norm, utils.py:124-133): one NVSwitch domain
     if 1 < world <= 8:
         from .comm_groups import CommGroup

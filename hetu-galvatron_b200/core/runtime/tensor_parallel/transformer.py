@@ -235,6 +235,129 @@ def _cp_attention(q, k, v, group, scale):
     return torch.cat(outs, 1)
 
 
+CP_COMM_MODES = ("allgather", "ring")
+
+
+def cp_comm_mode():
+    """``args.cp_comm``: how a context-parallel layer exchanges keys/values (``"allgather"``, the default, or ``"ring"``)."""
+    try:
+        from ..arguments import get_args
+        mode = getattr(get_args(), "cp_comm", "allgather")
+    except RuntimeError:
+        mode = "allgather"
+    if mode not in CP_COMM_MODES:
+        raise ValueError("cp_comm must be one of %s, not %r" % (", ".join(CP_COMM_MODES), mode))
+    return mode
+
+
+# ---- ring context parallelism (the reference's zigzag ring, transformer.py:2209-2551) ----------------------------------------
+# Rank r of c holds queries and keys of the zigzag chunks (r, 2c-1-r), s_loc/2 rows each.  Step i works on the K/V block of rank
+# j = (r - i) mod c, which reaches r after i hops: step 0 is local q x local K/V, causal; for j < r every query sees the block's
+# first chunk (chunk j) and nothing of its second; for j > r only the second query chunk (2c-1-r) sees the block, all of it.
+# The step functions below are generators that yield after every step: a model runs one rank's steps back to back, a test with
+# several ranks on one device interleaves them.  The transport (``ring``: send/recv/release of K/V and of the dK/dV accumulators)
+# is the only part that differs between backends.
+def _ring_block(r, j, half):
+    """-> (first query row, K/V rows used or None for all, causal) of the step that holds rank j's block"""
+    if j == r:
+        return 0, None, True
+    if j < r:
+        return 0, half, False
+    return half, None, False
+
+
+def run_steps(gen):
+    """drive a step generator to its end; -> its return value"""
+    while True:
+        try:
+            next(gen)
+        except StopIteration as stop:
+            return stop.value
+
+
+def ring_attention_fwd(be, ring, q, k, v, scale):
+    """-> (out [b, s_loc, n, d] bf16, lse [b, n, s_loc] fp32) of causal attention of the local queries over the whole sequence"""
+    c, r = ring.size, ring.rank
+    b, s, n, d = q.shape
+    half = s // 2
+    acc_out = torch.empty(b, s, n, d, dtype=torch.float32, device=q.device)
+    acc_lse = torch.empty(b, n, s, dtype=torch.float32, device=q.device)
+    out = torch.empty_like(q)
+    kv = (k, v)
+    for i in range(c):
+        if i > 0:
+            kv = ring.recv_kv(i)
+        if i < c - 1:
+            ring.send_kv(i, *kv)           # the next step's block travels while this step's attention runs
+        q0, nk, causal = _ring_block(r, (r - i) % c, half)
+        kb, vb = kv if nk is None else (kv[0][:, :nk], kv[1][:, :nk])
+        o, lse, _ = be.attention_fwd(q[:, q0:], kb, vb, causal, scale)
+        be.lse_merge(o, lse, acc_out, acc_lse, out if i == c - 1 else None, q0, init=i == 0)
+        if i > 0:
+            ring.release_kv(i)
+        yield
+    return out, acc_lse
+
+
+def ring_attention_bwd(be, ring, dout, q, k, v, out, lse, scale):
+    """-> (dq, dk, dv) bf16: the block backward of every step with the merged out / LSE; dq accumulates in fp32 here, dK/dV in the
+    fp32 accumulators that travel with the blocks and are back at their owner after the c-th hop"""
+    c, r = ring.size, ring.rank
+    b, s, n, d = q.shape
+    half = s // 2
+    dq_acc = torch.empty(b, s, n, d, dtype=torch.float32, device=q.device)
+    kv = (k, v)
+    for i in range(c):
+        if i > 0:
+            kv = ring.recv_kv(i)
+        if i < c - 1:
+            ring.send_kv(i, *kv)
+        q0, nk, causal = _ring_block(r, (r - i) % c, half)
+        kb, vb = kv if nk is None else (kv[0][:, :nk], kv[1][:, :nk])
+        lse_b = lse if q0 == 0 else lse[:, :, q0:].contiguous()
+        dq, dk, dv = be.attention_bwd(dout[:, q0:], q[:, q0:], kb, vb, out[:, q0:], lse_b, causal, scale, None)
+        if q0 == 0:
+            be.cast(dq, dq_acc, accumulate=i > 0)
+        else:
+            for bi in range(b):            # (rows q0.. of one sample are contiguous)
+                be.cast(dq[bi], dq_acc[bi, q0:], accumulate=True)
+        acc_in = ring.recv_acc(i) if i > 0 else None
+        ring.send_acc(i, acc_in, dk, dv, 0, s if nk is None else nk)
+        if i > 0:
+            ring.release_acc(i)
+            ring.release_kv(i)
+        yield
+    acc = ring.recv_acc(c)
+    dk_out, dv_out = torch.empty_like(k), torch.empty_like(v)
+    be.cast(acc[:k.numel()].view(k.shape), dk_out)
+    be.cast(acc[k.numel():].view(v.shape), dv_out)
+    ring.release_acc(c)
+    dq_out = torch.empty_like(q)
+    be.cast(dq_acc, dq_out)
+    return dq_out, dk_out, dv_out
+
+
+class _CpRingAttnFn(torch.autograd.Function):
+    """Causal self-attention under zigzag context parallelism over the ring: only this rank's K/V (s/c rows) is kept for
+    backward; the other blocks pass through the receive slots hop by hop, in the forward and again in the backward."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, group, scale):
+        be = get_backend()
+        ring = be.cp_ring(group)
+        out, lse = run_steps(ring_attention_fwd(be, ring, q, k, v, scale))
+        ctx.save_for_backward(q, k, v, out, lse)
+        ctx.group, ctx.scale = group, scale
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        q, k, v, out, lse = ctx.saved_tensors
+        be = get_backend()
+        dq, dk, dv = run_steps(ring_attention_bwd(be, be.cp_ring(ctx.group), dout.contiguous(), q, k, v, out, lse, ctx.scale))
+        return dq, dk, dv, None, None
+
+
 def _recompute_activations():
     try:
         from ..arguments import get_args
@@ -302,6 +425,7 @@ class ParallelAttention(nn.Module):
         if attention_type != AttnType.self_attn:
             raise NotImplementedError("only self attention is on the Galvatron hot path")
         self.use_cp = bool(use_zigzag_cp) or _size(cp_group) > 1
+        self.cp_comm = cp_comm_mode()
         if self.use_cp and use_ulysses and _size(sp_group) > 1:
             raise NotImplementedError("context parallelism together with Ulysses on the same layer is not supported")
         self.layer_number = max(1, layer_number)
@@ -377,7 +501,10 @@ class ParallelAttention(nn.Module):
             (ctxt,) = _UlyssesFn.apply(self.sp_group, False, ctxt)         # [b, s/p, n, hn]
         elif self.use_cp:
             assert causal, "context parallelism is implemented for causal self-attention"
-            ctxt = _cp_attention(q, k, v, self.cp_group, self.softmax_scale)   # [b, s/c, np, hn]
+            if self.cp_comm == "ring" and _size(self.cp_group) > 1:
+                ctxt = _CpRingAttnFn.apply(q, k, v, self.cp_group, self.softmax_scale)   # [b, s/c, np, hn]
+            else:
+                ctxt = _cp_attention(q, k, v, self.cp_group, self.softmax_scale)      # [b, s/c, np, hn]
         else:
             ctxt = self._core_attention(q, k, v, causal, key_mask)          # [b, s, np, hn]
         b, s = ctxt.shape[0], ctxt.shape[1]

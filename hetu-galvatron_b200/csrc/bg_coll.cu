@@ -534,6 +534,99 @@ __global__ void BG_SLIM all_to_all_rows_kernel(const __grid_constant__ A2AArgs a
     sync_peers<true, false, false>(s);
 }
 
+// ------------------------------------------------------------------------------------------------
+// C15: ring context parallelism -- one hop of K/V (bf16) or of the dK/dV accumulators (fp32) to the next cp member.
+// Flags: lane BG_LANE_RING of the group's pad, [channel][8] u32 per member: index kind*4 + parity = "a block arrived in my
+// slot[parity]" (raised by the previous member), kind*4 + 2 + parity = "the next member freed its slot[parity]" (raised by it).
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ int ring_next(const Sig& s) { return s.me + 1 == s.n ? 0 : s.me + 1; }
+__device__ __forceinline__ int ring_prev(const Sig& s) { return s.me == 0 ? s.n - 1 : s.me - 1; }
+
+// CTA-uniform: thread 0 waits for the receiver's "free" flag of this channel, the CTA stores its vector range, then thread 0 raises
+// the receiver's "arrived" flag after every thread's stores are visible at .sys scope
+__device__ __forceinline__ void ring_enter(const Sig& s, int kind, int parity, int wait_free) {
+    if (wait_free && threadIdx.x == 0) sig_spin_cas(s.local + blockIdx.x * BG_MAX_PEERS + kind * 4 + 2 + parity, 1u, 0u, false, s);
+    __syncthreads();
+}
+__device__ __forceinline__ void ring_leave(const Sig& s, int kind, int parity) {
+    __threadfence_system();
+    __syncthreads();
+    if (threadIdx.x == 0) sig_spin_cas(s.peer[ring_next(s)] + blockIdx.x * BG_MAX_PEERS + kind * 4 + parity, 0u, 1u, true, s);
+}
+
+// [k | v] -> the next member's slot; CTA b pushes the b-th contiguous range of the 2 * nvec 16-B vectors
+__global__ void BG_SLIM cp_ring_push_kernel(const uint4* __restrict__ k, const uint4* __restrict__ v, uint4* __restrict__ dst,
+                                           size_t nvec, int parity, int wait_free, const __grid_constant__ Sig s) {
+    ring_enter(s, 0, parity, wait_free);
+    const size_t total = 2 * nvec, per = (total + gridDim.x - 1) / gridDim.x;
+    const size_t lo = (size_t)blockIdx.x * per, hi = lo + per < total ? lo + per : total;
+    for (size_t i0 = lo + threadIdx.x; i0 < hi; i0 += (size_t)kThreads * kUnroll) {
+        uint4 regs[kUnroll];
+#pragma unroll
+        for (int u = 0; u < kUnroll; ++u) {
+            const size_t i = i0 + (size_t)u * kThreads;
+            if (i < hi) regs[u] = ld16_stream(i < nvec ? k + i : v + (i - nvec));
+        }
+#pragma unroll
+        for (int u = 0; u < kUnroll; ++u) {
+            const size_t i = i0 + (size_t)u * kThreads;
+            if (i < hi) st16(dst + i, regs[u]);
+        }
+    }
+    ring_leave(s, 0, parity);
+}
+
+struct RingAcc {
+    const float* acc_in;                 // this member's received accumulators [dK | dV] (nullptr at the first step)
+    const __nv_bfloat16* contrib[2];     // the step's dK, dV rows [batch][c_rows][row_elems]
+    float* dst;                          // the next member's slot [dK | dV]
+    long long rows, row_elems, c_row0, c_rows;
+    size_t units;                        // 8-element units per tensor
+};
+
+// next = acc_in + contribution, in that order, per element: the sum over the ring has one fixed order (owner, owner + 1, ...)
+__global__ void BG_SLIM cp_ring_acc_push_kernel(const __grid_constant__ RingAcc a, int parity, int wait_free, const __grid_constant__ Sig s) {
+    ring_enter(s, 1, parity, wait_free);
+    const size_t total = 2 * a.units, per = (total + gridDim.x - 1) / gridDim.x;
+    const size_t lo = (size_t)blockIdx.x * per, hi = lo + per < total ? lo + per : total;
+    const long long blk = a.rows * a.row_elems;
+    for (size_t u = lo + threadIdx.x; u < hi; u += kThreads) {
+        float f[8];
+        if (a.acc_in) {
+            const uint4 x = ld16_stream(a.acc_in + u * 8), y = ld16_stream(a.acc_in + u * 8 + 4);
+            f[0] = __uint_as_float(x.x); f[1] = __uint_as_float(x.y); f[2] = __uint_as_float(x.z); f[3] = __uint_as_float(x.w);
+            f[4] = __uint_as_float(y.x); f[5] = __uint_as_float(y.y); f[6] = __uint_as_float(y.z); f[7] = __uint_as_float(y.w);
+        } else {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) f[i] = 0.f;
+        }
+        const int t = u >= a.units;
+        const long long e = (long long)(u - (t ? a.units : 0)) * 8;
+        const long long bi = e / blk, rem = e - bi * blk, row = rem / a.row_elems;
+        if (row >= a.c_row0 && row < a.c_row0 + a.c_rows) {
+            float c[8];
+            unpack8(ld16_stream(a.contrib[t] + ((bi * a.c_rows + row - a.c_row0) * a.row_elems + (rem - row * a.row_elems))), c);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) f[i] += c[i];
+        }
+        st16(a.dst + u * 8, make_uint4(__float_as_uint(f[0]), __float_as_uint(f[1]), __float_as_uint(f[2]), __float_as_uint(f[3])));
+        st16(a.dst + u * 8 + 4, make_uint4(__float_as_uint(f[4]), __float_as_uint(f[5]), __float_as_uint(f[6]), __float_as_uint(f[7])));
+    }
+    ring_leave(s, 1, parity);
+}
+
+// consumer side, on the stream of the kernels that read the slot: wait for every channel's "arrived" flag ...
+__global__ void BG_SLIM cp_ring_wait_kernel(int kind, int parity, int channels, const __grid_constant__ Sig s) {
+    for (int ch = threadIdx.x; ch < channels; ch += kThreads)
+        sig_spin_cas(s.local + ch * BG_MAX_PEERS + kind * 4 + parity, 1u, 0u, false, s);
+}
+// ... and, once those kernels are done with it, hand the slot back to the previous member
+__global__ void BG_SLIM cp_ring_release_kernel(int kind, int parity, int channels, const __grid_constant__ Sig s) {
+    __threadfence_system();
+    for (int ch = threadIdx.x; ch < channels; ch += kThreads)
+        sig_spin_cas(s.peer[ring_prev(s)] + ch * BG_MAX_PEERS + kind * 4 + 2 + parity, 0u, 1u, true, s);
+}
+
 }  // namespace
 
 // Every kernel of this file is loaded up front (bg_ctx_create): with CUDA's lazy module loading the FIRST launch of a kernel
@@ -544,6 +637,10 @@ int bg_preload_coll() {
     const void* kernels[] = {
         K(coll_barrier_kernel),
         K(all_to_all_rows_kernel),
+        K(cp_ring_push_kernel),
+        K(cp_ring_acc_push_kernel),
+        K(cp_ring_wait_kernel),
+        K(cp_ring_release_kernel),
         K(all_reduce_nvls_kernel<true>),
         K(all_reduce_nvls_kernel<false>),
         K((all_gather_push_kernel<float, __nv_bfloat16, true>)),
@@ -817,6 +914,86 @@ extern "C" int bg_all_reduce_nvls(bg_ctx_t c, int gid, int lane, size_t byte_off
         all_reduce_nvls_kernel<true><<<grid, kThreads, 0, st>>>((char*)m.va + byte_offset, c->arena + m.arena_off + byte_offset, (char*)dst, vecs, scale, s);
     else
         all_reduce_nvls_kernel<false><<<grid, kThreads, 0, st>>>((char*)m.va + byte_offset, c->arena + m.arena_off + byte_offset, (char*)dst, vecs, scale, s);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// C15: ring context parallelism
+// ------------------------------------------------------------------------------------------------
+// channels of a hop: a function of the per-tensor element count only, so a push and its wait / release agree
+static int ring_channels(int kind, size_t elems) {
+    const size_t work = kind == 0 ? 2 * elems / 8 / kUnroll : 2 * elems / 8;
+    return comm_grid(work + 1, kThreads, 2);
+}
+
+static int ring_sig(bg_ctx_t c, int gid, int parity, Sig* s, const Group** g, int site) {
+    int rc = make_sig(c, gid, BG_LANE_RING, s, g);
+    if (rc) return rc;
+    if ((*g)->n < 2) return fail(BG_EINVAL, "cp ring: group of %d member(s)", (*g)->n);
+    if (parity != 0 && parity != 1) return fail(BG_EINVAL, "cp ring: parity %d", parity);
+    s->site = site;
+    BG_CUDA(cudaSetDevice(c->device));
+    return BG_OK;
+}
+
+extern "C" int bg_cp_ring_push(bg_ctx_t c, int gid, int parity, int wait_free, const void* k, const void* v, size_t elems,
+                               const size_t* slot_offs, void* stream) {
+    Sig s; const Group* g;
+    int rc = ring_sig(c, gid, parity, &s, &g, 13);
+    if (rc) return rc;
+    if (elems % 8 || (uintptr_t)k % 16 || (uintptr_t)v % 16) return fail(BG_EINVAL, "bg_cp_ring_push: elems %% 8, 16-B aligned k / v");
+    PeerPtrs dst;
+    rc = resolve(c, *g, slot_offs, 2 * elems * 2, &dst);
+    if (rc) return rc;
+    const int next = g->me + 1 == g->n ? 0 : g->me + 1;
+    cp_ring_push_kernel<<<ring_channels(0, elems), kThreads, 0, (cudaStream_t)stream>>>(
+        (const uint4*)k, (const uint4*)v, (uint4*)dst.p[next], elems / 8, parity, wait_free, s);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_cp_ring_acc_push(bg_ctx_t c, int gid, int parity, int wait_free, const float* acc_in, const void* dk, const void* dv,
+                                   long long batch, long long rows, long long row_elems, long long c_row0, long long c_rows,
+                                   const size_t* slot_offs, void* stream) {
+    Sig s; const Group* g;
+    int rc = ring_sig(c, gid, parity, &s, &g, 16);
+    if (rc) return rc;
+    if (batch < 1 || rows < 1 || row_elems < 8 || row_elems % 8 || c_row0 < 0 || c_rows < 0 || c_row0 + c_rows > rows)
+        return fail(BG_EINVAL, "bg_cp_ring_acc_push: bad shape (%lld, %lld, %lld) rows %lld+%lld", batch, rows, row_elems, c_row0, c_rows);
+    if ((uintptr_t)acc_in % 16 || (uintptr_t)dk % 16 || (uintptr_t)dv % 16 || (c_rows && (!dk || !dv)))
+        return fail(BG_EINVAL, "bg_cp_ring_acc_push: 16-B aligned operands");
+    const size_t elems = (size_t)(batch * rows * row_elems);
+    PeerPtrs dst;
+    rc = resolve(c, *g, slot_offs, 2 * elems * 4, &dst);
+    if (rc) return rc;
+    RingAcc a;
+    a.acc_in = acc_in;
+    a.contrib[0] = (const __nv_bfloat16*)dk; a.contrib[1] = (const __nv_bfloat16*)dv;
+    a.dst = (float*)dst.p[g->me + 1 == g->n ? 0 : g->me + 1];
+    a.rows = rows; a.row_elems = row_elems; a.c_row0 = c_row0; a.c_rows = c_rows;
+    a.units = elems / 8;
+    cp_ring_acc_push_kernel<<<ring_channels(1, elems), kThreads, 0, (cudaStream_t)stream>>>(a, parity, wait_free, s);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_cp_ring_wait(bg_ctx_t c, int gid, int kind, int parity, size_t elems, void* stream) {
+    Sig s; const Group* g;
+    int rc = ring_sig(c, gid, parity, &s, &g, 14);
+    if (rc) return rc;
+    if (kind != 0 && kind != 1) return fail(BG_EINVAL, "bg_cp_ring_wait: kind %d", kind);
+    cp_ring_wait_kernel<<<1, kThreads, 0, (cudaStream_t)stream>>>(kind, parity, ring_channels(kind, elems), s);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_cp_ring_release(bg_ctx_t c, int gid, int kind, int parity, size_t elems, void* stream) {
+    Sig s; const Group* g;
+    int rc = ring_sig(c, gid, parity, &s, &g, 15);
+    if (rc) return rc;
+    if (kind != 0 && kind != 1) return fail(BG_EINVAL, "bg_cp_ring_release: kind %d", kind);
+    cp_ring_release_kernel<<<1, kThreads, 0, (cudaStream_t)stream>>>(kind, parity, ring_channels(kind, elems), s);
     BG_CHECK_LAUNCH();
     return BG_OK;
 }

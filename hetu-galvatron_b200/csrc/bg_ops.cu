@@ -704,9 +704,81 @@ __global__ void __launch_bounds__(kCeThreads) ce_bwd_kernel(void* __restrict__ l
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// ring context parallelism: log-sum-exp merge of one block's attention result (transformer.py:2209-2250)
+// ---------------------------------------------------------------------------------------------
+// One thread per 8 head-dim elements of one (sample, query row, head); the d / 8 threads of a row sit in one warp.  Every thread
+// of a row reads the two LSEs, the warp synchronises, then the row's first thread writes the merged LSE.
+__global__ void __launch_bounds__(kThreads) lse_merge_kernel(const uint4* __restrict__ blk_out, const float* __restrict__ blk_lse,
+                                                             float* __restrict__ acc_out, float* __restrict__ acc_lse,
+                                                             uint4* __restrict__ final_out, long long s, long long sq_blk, long long n,
+                                                             int vpr, long long row_off, long long rows_total, int init) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool ok = idx < rows_total * vpr;
+    const long long row = ok ? idx / vpr : 0, part = idx - row * vpr;      // row = (bi * s + q) * n + h
+    const long long h = row % n, q = (row / n) % s, bi = row / (n * s);
+    const bool in_blk = ok && q >= row_off && q < row_off + sq_blk;
+    const long long qb = q - row_off;
+    float la = -INFINITY, lb = -INFINITY;
+    if (in_blk) {
+        lb = blk_lse[(bi * n + h) * sq_blk + qb];
+        if (!init) la = acc_lse[(bi * n + h) * s + q];
+    }
+    __syncwarp();
+    if (!ok) return;
+    float4* ao = reinterpret_cast<float4*>(acc_out) + idx * 2;
+    float f[8];
+    if (in_blk) {
+        float b8[8];
+        unpack8(ld16_stream(blk_out + ((bi * sq_blk + qb) * n + h) * vpr + part), b8);
+        float wa = 0.f, wb = 1.f, lse = lb;
+        if (!init) {
+            const float m = fmaxf(la, lb);
+            if (m == -INFINITY) {
+                wb = 0.f;
+            } else {
+                lse = m + logf(expf(la - m) + expf(lb - m));
+                wa = expf(la - lse);
+                wb = expf(lb - lse);
+            }
+        }
+        if (init) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) f[i] = b8[i];
+        } else {
+            const float4 x = ao[0], y = ao[1];
+            f[0] = x.x * wa + b8[0] * wb; f[1] = x.y * wa + b8[1] * wb; f[2] = x.z * wa + b8[2] * wb; f[3] = x.w * wa + b8[3] * wb;
+            f[4] = y.x * wa + b8[4] * wb; f[5] = y.y * wa + b8[5] * wb; f[6] = y.z * wa + b8[6] * wb; f[7] = y.w * wa + b8[7] * wb;
+        }
+        ao[0] = make_float4(f[0], f[1], f[2], f[3]);
+        ao[1] = make_float4(f[4], f[5], f[6], f[7]);
+        if (part == 0) acc_lse[(bi * n + h) * s + q] = lse;
+    } else if (final_out) {
+        const float4 x = ao[0], y = ao[1];
+        f[0] = x.x; f[1] = x.y; f[2] = x.z; f[3] = x.w; f[4] = y.x; f[5] = y.y; f[6] = y.z; f[7] = y.w;
+    }
+    if (final_out) st16(final_out + idx, pack8(f));
+}
+
 }  // namespace
 
 #define BG_ALIGNED16(p) (((uintptr_t)(p) % 16) == 0)
+
+extern "C" int bg_lse_merge(const void* blk_out, const float* blk_lse, float* acc_out, float* acc_lse, void* final_out, long long b,
+                            long long s, long long sq_blk, long long n, long long d, long long row_off, int init, void* stream) {
+    if (b < 1 || s < 1 || n < 1 || d < 8 || d % 8 || d > 256 || 32 % (d / 8) || sq_blk < 1 || row_off < 0 || row_off + sq_blk > s)
+        return fail(BG_EINVAL, "bg_lse_merge: bad shape b %lld s %lld sq_blk %lld n %lld d %lld row_off %lld", b, s, sq_blk, n, d, row_off);
+    if (init && (row_off != 0 || sq_blk != s)) return fail(BG_EINVAL, "bg_lse_merge: init needs a block of every row");
+    if (!BG_ALIGNED16(blk_out) || !BG_ALIGNED16(acc_out) || !BG_ALIGNED16(final_out))
+        return fail(BG_EINVAL, "bg_lse_merge: pointers must be 16-B aligned");
+    const int vpr = (int)(d / 8);
+    const long long rows = b * s * n, threads = rows * vpr;
+    const int grid = (int)((threads + kThreads - 1) / kThreads);
+    lse_merge_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const uint4*)blk_out, blk_lse, acc_out, acc_lse, (uint4*)final_out, s,
+                                                                 sq_blk, n, vpr, row_off, rows, init);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
 
 extern "C" int bg_cast(const void* src, int src_dtype, void* dst, int dst_dtype, size_t elems, float scale, int accumulate,
                        void* stream) {

@@ -30,7 +30,7 @@ extern "C" {
 #define BG_ABI_VERSION 1
 #define BG_MAX_PEERS 8      /* one NVSwitch domain */
 #define BG_MAX_WORLD 64
-#define BG_LANES 6          /* independent barrier lanes per group: unshard / grad-reduce / activations / misc / fused-op push / spare */
+#define BG_LANES 6          /* independent barrier lanes per group: unshard / grad-reduce / activations / misc / fused-op push / cp ring */
 #define BG_MAX_CHANNELS 256 /* max CTAs of a cross-rank kernel (one barrier channel per CTA; the default is one slim CTA per SM) */
 
 typedef struct bg_ctx* bg_ctx_t;
@@ -75,7 +75,8 @@ int bg_ctx_error_flag(bg_ctx_t ctx, int* flag);                         /* devic
 /* info8[0] = status; [1] = kind (1 signalling a peer, 2 waiting for a peer, 3 fused-GEMM tile reducer);
  * [2] = CTA; [3] = thread or tile; [4] = value last seen; [5], [6] = group index/size or expected count/tiles;
  * [7] = launch site of a barrier timeout (1 all-gather, 2 reduce-scatter, 3 all-reduce, 6 all-to-all, 7 entry barrier of a fused
- * GEMM, 8 exit barrier of the all-reduce tile reducer, 10/11 p2p flags, 12 push kernel of the fused all-gather+GEMM), kind 4 = the
+ * GEMM, 8 exit barrier of the all-reduce tile reducer, 10/11 p2p flags, 12 push kernel of the fused all-gather+GEMM, 13 cp ring
+ * K/V push, 14 cp ring wait, 15 cp ring release, 16 cp ring accumulate-and-forward push), kind 4 = the
  * gathering GEMM's TMA producer waiting for a block.
  * The reference's analogue is the NCCL watchdog's timeout dump (ProcessGroupNCCL); here a lost peer traps the
  * kernel and leaves this record in mapped host memory. */
@@ -151,6 +152,30 @@ int bg_p2p_send(bg_ctx_t ctx, int peer_rank, size_t dst_off, const void* src, si
 int bg_p2p_wait(bg_ctx_t ctx, int peer_rank, int flag_id, void* stream);
 int bg_p2p_release(bg_ctx_t ctx, int peer_rank, int flag_id, void* stream);
 
+/* C15  ring context parallelism: one hop of the zigzag ring (transformer.py:2252-2334 RingComm send_recv / commit / wait, which
+ * the forward and backward schedules of :2335-2551 call once per step).  Member i of the cp group sends to member i+1 (mod n).
+ * Receive slots are double-buffered by step parity; the flags live in the group's barrier lane BG_LANE_RING, one per CTA channel:
+ * a push CTA waits for the receiver's "slot free" flag (skipped with wait_free = 0: the slot's first use), stores 16-B vectors into
+ * the receiver's slot and raises its "arrived" flag; bg_cp_ring_wait consumes every channel's "arrived" flag on the receiver's
+ * stream, bg_cp_ring_release raises the sender's "slot free" flags once the slot has been read.  The flags reset themselves
+ * (CAS 0->1 / 1->0); spin timeouts leave the who/where record of bg_ctx_error_info (sites 13-16).  `elems` (per tensor) fixes the
+ * number of channels, so a push and its wait / release must pass the same value.
+ * kind 0: K and V, bf16: slot = [k | v] (elems each).  slot_offs: the group's symmetric buffer offsets of the parity's slot. */
+#define BG_LANE_RING 5
+int bg_cp_ring_push(bg_ctx_t ctx, int gid, int parity, int wait_free, const void* k, const void* v, size_t elems,
+                    const size_t* slot_offs, void* stream);
+/* kind 1: the backward's dK / dV accumulators, fp32, accumulate-and-forward (transformer.py:2470-2540, where the reference adds the
+ * received fp32 buffers and the step's gradients on the compute stream before sending):
+ *     next_slot[t] = (acc_in ? acc_in[t] : 0) + (float)contribution_t
+ * for t in {dK, dV}; both are [batch][rows][row_elems] with the contribution [batch][c_rows][row_elems] bf16 covering rows
+ * c_row0 .. c_row0 + c_rows - 1 only (c_rows 0: none).  The sum happens inside the push, fixed order: results are deterministic. */
+int bg_cp_ring_acc_push(bg_ctx_t ctx, int gid, int parity, int wait_free, const float* acc_in, const void* dk, const void* dv,
+                        long long batch, long long rows, long long row_elems, long long c_row0, long long c_rows,
+                        const size_t* slot_offs, void* stream);
+/* kind 0 / 1 as above; elems = per-tensor elements of the push being waited for / released */
+int bg_cp_ring_wait(bg_ctx_t ctx, int gid, int kind, int parity, size_t elems, void* stream);
+int bg_cp_ring_release(bg_ctx_t ctx, int gid, int kind, int parity, size_t elems, void* stream);
+
 /* ---- local fused elementwise ops adjacent to the collectives (K5/K6/K9/a10 in SURVEY 2.3) ------------------ */
 int bg_cast(const void* src, int src_dtype, void* dst, int dst_dtype, size_t elems, float scale, int accumulate,
             void* stream);
@@ -186,6 +211,14 @@ int bg_dropout_bwd(const void* dy, void* dx, float* dbias_partial, int n_partial
 /* host-only: one Philox4x32-10 block (the generator of curand_philox4x32_x.h), so the mask definition can be checked without a
  * GPU.  No CUDA call. */
 void bg_philox4x32_10(const uint32_t ctr[4], const uint32_t key[2], uint32_t out[4]);
+/* log-sum-exp merge of one ring step's flash-attn block result into the running result (transformer.py:2209-2250
+ * update_out_and_lse): for query rows row_off .. row_off + sq_blk - 1 of the running state,
+ *     lse = m + log(exp(lse_a - m) + exp(lse_b - m)),  m = max(lse_a, lse_b);   out = out_a exp(lse_a - lse) + out_b exp(lse_b - lse)
+ * in fp32.  blk_out [b][sq_blk][n][d] bf16, blk_lse [b][n][sq_blk] fp32 (flash-attn's layout); acc_out [b][s][n][d] fp32 and
+ * acc_lse [b][n][s] fp32 are updated in place (init = 1: they are set to the block instead).  final_out (bf16 [b][s][n][d], may be
+ * NULL): also write every row of the merged output there, rounded once; acc_lse is then the output's LSE.  d % 8 == 0, d <= 256. */
+int bg_lse_merge(const void* blk_out, const float* blk_lse, float* acc_out, float* acc_lse, void* final_out, long long b, long long s,
+                 long long sq_blk, long long n, long long d, long long row_off, int init, void* stream);
 int bg_swiglu_fwd(const void* gate_up, void* y, long long rows, long long ffn, void* stream);
 int bg_swiglu_bwd(const void* dy, const void* gate_up, void* dgate_up, long long rows, long long ffn, void* stream);
 /* fused QKV split + RoPE + [s,b,ng,(r+2)*hn] -> q [b,s,ng*r,hn], k/v [b,s,ng,hn] relayout; backward=1 is the exact

@@ -1,5 +1,5 @@
 """Micro-benchmarks of the C-ABI kernels on one GPU (CUDA events, warm-up, L2-exceeding inputs).
-Usage: python scripts/bench_kernels.py [gemm] [cast] [ops] [attn] [dropout]  -> JSON lines on stdout."""
+Usage: python scripts/bench_kernels.py [gemm] [cast] [ops] [attn] [dropout] [cp]  -> JSON lines on stdout."""
 import json
 import os
 import sys
@@ -282,6 +282,121 @@ def dropout():
         print(json.dumps({"bench": "sdpa_dropout_backends", "shape": name, "accepts_dropout": ok}), flush=True)
         del sets, masks
         torch.cuda.empty_cache()
+    be.close()
+
+
+class _LocalRing:
+    """Stand-in ring transport that moves nothing: every block is the rank's own (same shapes as the real hops), so the ring
+    schedule of tensor_parallel/transformer.py runs its attention, merge and cast work with the transport excluded."""
+
+    def __init__(self, c, k, v):
+        self.size, self.rank, self.kv = c, 0, (k, v)
+        self.acc = torch.zeros(2 * k.numel(), device=k.device)
+
+    def send_kv(self, step, k, v):
+        pass
+
+    def recv_kv(self, step):
+        return self.kv
+
+    def release_kv(self, step):
+        pass
+
+    def send_acc(self, step, acc_in, dk, dv, c_row0, c_rows):
+        pass
+
+    def recv_acc(self, step):
+        return self.acc
+
+    def release_acc(self, step):
+        pass
+
+
+def cp():
+    """Ring context parallelism at Llama-3.2-1B attention shapes (32 heads, 8 KV heads of 64), microbatch 1, sequence S in {32k, 128k},
+    cp degree c in {2, 4, 8}.  Per rank: attention forward + backward of the ring schedule (2c-1 flash-attn block calls, the LSE
+    merges and the fp32 accumulation casts; transport excluded) against the all-gather path's two prefix calls on the gathered
+    sequence (gather excluded); the merge and the two push kernels in GB/s over algorithmic bytes -- the pushes between two virtual
+    ranks on this one device, i.e. through local HBM, not NVLink; and the K/V bytes each path keeps for backward per layer."""
+    import subprocess
+    from flash_attn import flash_attn_func
+    from hetu_galvatron_b200.core.runtime.backend import CudaBackend, _CpRing
+    from hetu_galvatron_b200.core.runtime.comm_groups import CommGroup
+    from hetu_galvatron_b200.core.runtime.tensor_parallel import transformer as tr
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    print(json.dumps({"nvidia_smi": q.stdout.strip()}), flush=True)
+    n, ng, d, b = 32, 8, 64, 1
+    scale = d ** -0.5
+    be = CudaBackend(arena_bytes=1 << 24)
+    for S in (32768, 131072):
+        for c in (2, 4, 8):
+            s = S // c
+            qq = torch.randn(b, s, n, d, device="cuda").to(BF)
+            k, v = [torch.randn(b, s, ng, d, device="cuda").to(BF) for _ in range(2)]
+            do = torch.randn(b, s, n, d, device="cuda").to(BF)
+            ring = _LocalRing(c, k, v)
+
+            def ring_fb():
+                out, lse = tr.run_steps(tr.ring_attention_fwd(be, ring, qq, k, v, scale))
+                tr.run_steps(tr.ring_attention_bwd(be, ring, do, qq, k, v, out, lse, scale))
+            kf, vf = [torch.randn(b, S, ng, d, device="cuda").to(BF).requires_grad_(True) for _ in range(2)]
+            qg = qq.detach().clone().requires_grad_(True)
+            half = s // 2
+
+            def gather_fb():
+                outs = [flash_attn_func(qg[:, :half], kf[:, :(ch + 1) * half], vf[:, :(ch + 1) * half], softmax_scale=scale, causal=True)
+                        for ch in (0, 2 * c - 1)]     # rank 0's chunks
+                torch.cat(outs, 1).backward(do)
+            iters = 3 if S > 32768 else 10
+            t_ring, t_gather = [], []
+            for _ in range(3):                       # interleaved rounds
+                t_ring.append(timeit(ring_fb, iters=iters, warm=1))
+                t_gather.append(timeit(gather_fb, iters=iters, warm=1))
+            kv_ring, kv_gather = 2 * b * s * ng * d * 2, 2 * b * S * ng * d * 2
+            print(json.dumps({"bench": "cp_attention_fwd_bwd_per_rank", "S": S, "c": c, "ring_ms": round(sorted(t_ring)[1], 3),
+                              "gather_ms": round(sorted(t_gather)[1], 3), "ring_over_gather": round(sorted(t_ring)[1] / sorted(t_gather)[1], 3),
+                              "spread_pct": round(100 * (max(t_ring + t_gather) - min(t_ring + t_gather)) / min(t_ring + t_gather), 1),
+                              "transport": "excluded (both paths)", "kv_kept_for_backward_MiB_ring": round(kv_ring / 2 ** 20, 1),
+                              "kv_kept_for_backward_MiB_gather": round(kv_gather / 2 ** 20, 1)}), flush=True)
+            # the merge: a full-rows step (read block out bf16 + block LSE, read/write running out + LSE fp32)
+            acc_out, acc_lse = torch.randn(b, s, n, d, device="cuda"), torch.randn(b, n, s, device="cuda")
+            blk_lse = torch.randn(b, n, s, device="cuda")
+            t = timeit(lambda: bg.lse_merge(qq, blk_lse, acc_out, acc_lse), iters=20)
+            nbytes = b * s * n * d * (2 + 8) + b * n * s * 12
+            print(json.dumps({"bench": "cp_lse_merge", "S": S, "c": c, "ms": round(t, 4), "GBps_algorithmic": round(nbytes / t / 1e6, 1),
+                              "pct_of_3350GBps": round(100 * nbytes / t / 1e6 / 3350, 1)}), flush=True)
+            del qq, do, kf, vf, qg, acc_out, acc_lse, ring
+            # the pushes, between two virtual ranks on this device
+            elems = b * s * ng * d
+            comms = bg.BgComm.local_world(2, device=0, arena_bytes=_CpRing.slot_bytes(elems) + (16 << 20))
+            group = CommGroup([0, 1])
+            bufs = [cm.sym_alloc(group, _CpRing.slot_bytes(elems)) for cm in comms]
+            for cm in comms:
+                cm.exchange()
+            rings = [_CpRing(cm, group, buf, elems) for cm, buf in zip(comms, bufs)]
+            dk, dv = [torch.randn(b, s, ng, d, device="cuda").to(BF) for _ in range(2)]
+
+            def hop_kv():
+                rings[0].send_kv(0, k, v)
+                rings[1].recv_kv(1)
+                rings[1].release_kv(1)
+
+            def hop_acc():
+                rings[0].send_acc(0, None, dk, dv, 0, s)
+                rings[1].recv_acc(1)
+                rings[1].release_acc(1)
+            rings[1].shape = tuple(k.shape)
+            for name, fn, nb in (("kv_push", hop_kv, 2 * elems * 2), ("acc_push", hop_acc, 2 * elems * (2 + 4))):
+                t = timeit(fn, iters=20)
+                print(json.dumps({"bench": "cp_ring_" + name, "S": S, "c": c, "ms_per_hop": round(t, 4),
+                                  "GBps_algorithmic": round(nb / t / 1e6, 1), "path": "local HBM (two virtual ranks on one device), not NVLink",
+                                  "bytes": "kv: K+V bf16 payload; acc: bf16 contribution read + fp32 accumulator written"}), flush=True)
+            torch.cuda.synchronize()
+            for cm in comms:
+                assert cm.error_flag() == 0
+                cm.close()
+            del k, v, dk, dv
+            torch.cuda.empty_cache()
     be.close()
 
 
