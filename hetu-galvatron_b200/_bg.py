@@ -69,6 +69,10 @@ SIGNATURES = {
     "bg_reduce_scatter_acc": (_i, [_vp, _i, _i, _c.POINTER(_sz), _i, _vp, _i, _sz, _f, _f, _i, _vp]),
     "bg_all_reduce": (_i, [_vp, _i, _i, _c.POINTER(_sz), _vp, _sz, _i, _i, _f, _vp]),
     "bg_reduce_scatter_adamw": (_i, [_vp, _i, _i, _c.POINTER(_sz), _i, _vp, _vp, _vp, _sz, _f, _f, _f, _f, _f, _f, _f, _ll, _vp]),
+    "bg_reduce_scatter_sumsq": (_i, [_vp, _i, _i, _c.POINTER(_sz), _i, _vp, _sz, _f, _f, _vp, _i, _c.POINTER(_sz), _i, _vp]),
+    "bg_reduce_scatter_adamw_clipped": (_i, [_vp, _i, _i, _c.POINTER(_sz), _i, _vp, _vp, _vp, _sz, _f, _f, _f, _f, _f, _f, _f, _ll, _vp,
+                                             _vp]),
+    "bg_adamw_clipped": (_i, [_vp, _vp, _vp, _vp, _sz, _f, _f, _f, _f, _f, _ll, _vp, _vp]),
     "bg_all_to_all_rows": (_i, [_vp, _i, _i, _c.POINTER(bg_a2a_desc), _i, _i, _vp]),
     "bg_p2p_send": (_i, [_vp, _i, _sz, _vp, _sz, _i, _vp]),
     "bg_p2p_wait": (_i, [_vp, _i, _i, _vp]),
@@ -538,6 +542,27 @@ class BgComm:
                                                 float(lr), float(beta1), float(beta2), float(eps), float(weight_decay), int(step),
                                                 sp))
 
+    def reduce_scatter_sumsq(self, group, src, src_dtype, shard_elems, prescale, postscale, partials, skip=(), dst=None,
+                             lane=LANE_REDUCE, stream=None):
+        """Norm pass: per-warp fp32 sums of squares of the reduced gradient into ``partials`` (fp32, whole tensor: the unused tail is
+        zeroed), leaving out the shard-relative element ranges ``skip`` [(lo, hi)]; with ``dst`` also the reduced fp32 shard."""
+        flat = [int(x) for r in skip for x in r]
+        arr = (_sz * max(1, len(flat)))(*flat)
+        with self._in_order(stream) as sp:
+            check(lib().bg_reduce_scatter_sumsq(self._ctx, self.group_id(group), lane, src.offs(), dtype_code(src_dtype),
+                                                _ptr(dst) if dst is not None else None, int(shard_elems), float(prescale),
+                                                float(postscale), _ptr(partials), partials.numel(), arr, len(skip), sp))
+
+    def reduce_scatter_adamw_clipped(self, group, src, src_dtype, param, exp_avg, exp_avg_sq, shard_elems, prescale, postscale, lr,
+                                     beta1, beta2, eps, weight_decay, step, clip_coef, lane=LANE_REDUCE, stream=None):
+        """``reduce_scatter_adamw`` with the gradient multiplied by the device scalar ``clip_coef`` (fp32 tensor, or None for 1)."""
+        with self._in_order(stream) as sp:
+            check(lib().bg_reduce_scatter_adamw_clipped(self._ctx, self.group_id(group), lane, src.offs(), dtype_code(src_dtype),
+                                                        _ptr(param), _ptr(exp_avg), _ptr(exp_avg_sq), int(shard_elems), float(prescale),
+                                                        float(postscale), float(lr), float(beta1), float(beta2), float(eps),
+                                                        float(weight_decay), int(step),
+                                                        _ptr(clip_coef) if clip_coef is not None else None, sp))
+
     def all_reduce(self, group, src, dst, elems=None, op=SUM, scale=1.0, lane=LANE_ACT, stream=None, src_byte_offset=0):
         n = dst.numel() if elems is None else int(elems)
         offs = src.offs() if src_byte_offset == 0 else src.sub(src_byte_offset)
@@ -630,6 +655,13 @@ class BgComm:
 def cast(src, dst, scale=1.0, accumulate=False, stream=None):
     check(lib().bg_cast(_ptr(src), dtype_code(src.dtype), _ptr(dst), dtype_code(dst.dtype), src.numel(), float(scale),
                         1 if accumulate else 0, _stream_ptr(stream)))
+
+
+def adamw_clipped(param, exp_avg, exp_avg_sq, grad, lr, beta1, beta2, eps, weight_decay, step, clip_coef, stream=None):
+    """AdamW on fp32 (param, exp_avg, exp_avg_sq) with the local fp32 ``grad`` multiplied by the device scalar ``clip_coef``."""
+    check(lib().bg_adamw_clipped(_ptr(param), _ptr(exp_avg), _ptr(exp_avg_sq), _ptr(grad), grad.numel(), float(lr), float(beta1),
+                                 float(beta2), float(eps), float(weight_decay), int(step),
+                                 _ptr(clip_coef) if clip_coef is not None else None, _stream_ptr(stream)))
 
 
 def lse_merge(blk_out, blk_lse, acc_out, acc_lse, final_out=None, row_off=0, init=False, stream=None):

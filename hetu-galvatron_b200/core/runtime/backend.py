@@ -259,8 +259,9 @@ class CudaBackend:
                                      lane=self.bg.LANE_REDUCE)
                 self.cast(tmp, unit.master_grad, accumulate=accumulate)
 
-    def unit_reduce_adamw(self, unit, opt):
-        """C2 with the AdamW epilogue (reduce stream): gradients are consumed in registers, no fp32 gradient shard."""
+    def unit_reduce_adamw(self, unit, opt, clip_coef=None):
+        """C2 with the AdamW epilogue (reduce stream): gradients are consumed in registers, no fp32 gradient shard.  ``clip_coef``
+        (fp32 device scalar): the step pass of deferred clipping, the reduced gradient multiplied by it."""
         lr, b1, b2, eps, wd, step = opt.hyper()
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream())
@@ -268,9 +269,41 @@ class CudaBackend:
             self.reduce_stream.wait_event(ev)
             d, gsz = unit.group.size, (4 if unit.reduce_dtype == torch.float32 else 2)
             with self._timed("sdp_reduce_scatter_adamw", (d - 1) / d * unit.padded * gsz, self.reduce_stream):
-                self.comm.reduce_scatter_adamw(unit.group, unit.G, unit.reduce_dtype, unit.flat_param.data, unit.exp_avg, unit.exp_avg_sq,
-                                               unit.shard_elems, 1.0 / unit.prediv, 1.0 / unit.postdiv, lr, b1, b2, eps, wd, step,
+                if clip_coef is None:
+                    self.comm.reduce_scatter_adamw(unit.group, unit.G, unit.reduce_dtype, unit.flat_param.data, unit.exp_avg,
+                                                   unit.exp_avg_sq, unit.shard_elems, 1.0 / unit.prediv, 1.0 / unit.postdiv, lr, b1, b2,
+                                                   eps, wd, step, lane=self.bg.LANE_REDUCE)
+                else:
+                    self.comm.reduce_scatter_adamw_clipped(unit.group, unit.G, unit.reduce_dtype, unit.flat_param.data, unit.exp_avg,
+                                                           unit.exp_avg_sq, unit.shard_elems, 1.0 / unit.prediv, 1.0 / unit.postdiv, lr,
+                                                           b1, b2, eps, wd, step, clip_coef, lane=self.bg.LANE_REDUCE)
+                    self.n_fused["rs_adamw_clipped"] = self.n_fused.get("rs_adamw_clipped", 0) + 1
+
+    def clip_partials(self, n_units):
+        """Zeroed fp32 [n_units, k]: one row per unit for the norm pass's per-warp sums of squares (4 warps x the largest grid)."""
+        k = 4 * max(self.bg.get_tunable("comm_ctas"), self.bg.get_tunable("local_ctas"))
+        return torch.zeros(n_units, k, dtype=torch.float32, device=self.device)
+
+    def unit_reduce_sumsq(self, unit, partials, skip, into_master=False):
+        """Norm pass of deferred clipping (reduce stream): the unit's reduce-scatter, whose epilogue only writes the per-warp sums of
+        squares of the reduced gradient into ``partials`` (leaving out the shard-relative ranges ``skip``); ``into_master``: also
+        the fp32 gradient shard (units whose G cannot be read again at the step)."""
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream())
+        with torch.cuda.stream(self.reduce_stream):
+            self.reduce_stream.wait_event(ev)
+            d, gsz = unit.group.size, (4 if unit.reduce_dtype == torch.float32 else 2)
+            with self._timed("sdp_reduce_scatter_sumsq", (d - 1) / d * unit.padded * gsz, self.reduce_stream):
+                self.comm.reduce_scatter_sumsq(unit.group, unit.G, unit.reduce_dtype, unit.shard_elems, 1.0 / unit.prediv,
+                                               1.0 / unit.postdiv, partials, skip, dst=unit.master_grad if into_master else None,
                                                lane=self.bg.LANE_REDUCE)
+        self.n_fused["rs_sumsq"] = self.n_fused.get("rs_sumsq", 0) + 1
+
+    def unit_adamw_clipped(self, unit, opt, clip_coef):
+        """The clipped AdamW step on the unit's fp32 gradient shard (current stream, after ``finish_reductions``)."""
+        lr, b1, b2, eps, wd, step = opt.hyper()
+        self.bg.adamw_clipped(unit.flat_param.data, unit.exp_avg, unit.exp_avg_sq, unit.master_grad, lr, b1, b2, eps, wd, step, clip_coef)
+        self.n_fused["adamw_clipped"] = self.n_fused.get("adamw_clipped", 0) + 1
 
     def finish_reductions(self):
         torch.cuda.current_stream().wait_stream(self.reduce_stream)

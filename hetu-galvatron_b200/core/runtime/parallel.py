@@ -166,7 +166,8 @@ class ShardedUnit:
             master = full[self.rank_in_group * self.shard_elems:(self.rank_in_group + 1) * self.shard_elems].clone()
         self.flat_param = nn.Parameter(master, requires_grad=True)
         self.flat_param._bg_unit = self
-        self._master_grad = None       # fp32 gradient shard: allocated on first use (never, with the fused optimizer)
+        # fp32 gradient shard: allocated on first use (never with the fused optimizer, except for pooled zero3 units under clipping)
+        self._master_grad = None
         self.fused_opt = None          # set by FusedShardedAdamW: the reduction's epilogue applies the update
 
         # ---- peer-visible flat buffers: W (gathered params) and G (unsharded grads) --------------------------------
@@ -395,7 +396,10 @@ class ShardedUnit:
         if self.uses_fused_optimizer():
             if self._reduced_this_step:
                 raise RuntimeError("the fused optimizer needs one gradient reduction per step (async_grad_reduce)")
-            self.be.unit_reduce_adamw(self, self.fused_opt)
+            if self.fused_opt.deferred:     # clipping: only the norm pass now, the update at optimizer.step()
+                self.fused_opt.norm_pass(self)
+            else:
+                self.be.unit_reduce_adamw(self, self.fused_opt)
         else:
             self.be.unit_reduce(self, accumulate=self._reduced_this_step)
             self.flat_param.grad = self.master_grad

@@ -13,14 +13,22 @@ class FusedShardedAdamW(torch.optim.Optimizer):
     backward of the step finishes, ONE kernel pulls the peers' gradient slices, sums them and applies the AdamW step to
     the fp32 shard -- the fp32 gradient buffer is never materialised (30 GiB less at Llama-3-8B on one GPU) and the
     optimizer's own pass over the state disappears.  ``step()`` only advances the step counter and fences the reduce
-    stream; hyper-parameters take effect for the NEXT forward_backward.  Same rule as torch.optim.AdamW."""
+    stream; hyper-parameters take effect for the NEXT forward_backward.  Same rule as torch.optim.AdamW.
 
-    def __init__(self, model, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01):
+    ``clip_grad`` > 0 (Megatron's ``--clip-grad``) defers the update so that ``clip_grad_norm`` can scale it by the job-wide
+    gradient norm, still without an fp32 gradient buffer: the layer's reduction at the end of its backward becomes a norm pass
+    (the same reduce-scatter, whose epilogue only writes per-warp sums of squares of the reduced gradient), and ``step()``
+    re-runs the AdamW reduce-scatter over the untouched unsharded gradient with the clip coefficient, a device scalar that
+    ``clip_grad_norm`` sets and ``step()`` resets to 1.  Pooled zero3 units hand their gradient buffer back after the
+    reduction: their norm pass also writes the fp32 gradient shard, and ``step()`` applies the same clipped rule to it."""
+
+    def __init__(self, model, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01, clip_grad=0.0):
         params = list(model.parameters())
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
         self.units = list(model.model.units)
         self.step_count = 0
         self._fallback = None
+        self.deferred = clip_grad > 0
         plain = []
         for u in self.units:
             u.fused_opt = self
@@ -29,6 +37,14 @@ class FusedShardedAdamW(torch.optim.Optimizer):
                 u.exp_avg_sq = torch.zeros_like(u.flat_param.data)
             else:
                 plain.append(u.flat_param)
+        if self.deferred:
+            from .backend import get_backend
+            be = get_backend()
+            self.partials = be.clip_partials(len(self.units))      # row i: unit i's sums of squares of this step
+            self.clip_coef = torch.ones((), dtype=torch.float32, device=self.partials.device)
+            self._row = {id(u): i for i, u in enumerate(self.units)}
+            self._skip = {id(u): _shard_skip_ranges(u, be.rank) for u in self.units if u.uses_fused_optimizer()}
+            self._stepping = []         # units whose norm pass ran this step, in reduction order: their step passes
         if plain:   # replicated DDP layers: ordinary AdamW on their fp32 gradients
             g = self.param_groups[0]
             self._fallback = torch.optim.AdamW(plain, lr=g["lr"], betas=g["betas"], eps=g["eps"], weight_decay=g["weight_decay"],
@@ -38,10 +54,33 @@ class FusedShardedAdamW(torch.optim.Optimizer):
         g = self.param_groups[0]
         return g["lr"], g["betas"][0], g["betas"][1], g["eps"], g["weight_decay"], self.step_count + 1
 
+    def norm_pass(self, unit):
+        """Deferred clipping: the unit's reduction at the end of its backward (called by ``ShardedUnit.reduce_now``)."""
+        unit.be.unit_reduce_sumsq(unit, self.partials[self._row[id(unit)]], self._skip[id(unit)], into_master=unit.g_pool is not None)
+        self._stepping.append(unit)
+
+    def sum_of_squares(self):
+        """Device scalar: the sum of squares of this rank's share of the fused units' gradients, as the next update will see
+        them (scaled by the clip coefficient set so far)."""
+        return self.partials.sum() * self.clip_coef * self.clip_coef
+
     @torch.no_grad()
     def step(self, closure=None):
         from .backend import get_backend
-        get_backend().finish_reductions()
+        be = get_backend()
+        be.finish_reductions()
+        if self.deferred:
+            # the step passes, in the order of the norm passes (the same on every member of each group: they are collectives)
+            for u in self._stepping:
+                if u.g_pool is not None:
+                    be.unit_adamw_clipped(u, self, self.clip_coef)
+                else:
+                    be.unit_reduce_adamw(u, self, clip_coef=self.clip_coef)
+                    u._reduce_event = be.reduce_done_event()      # the next backward may overwrite G only after this read
+            self._stepping = []
+            be.finish_reductions()
+            self.partials.zero_()
+            self.clip_coef.fill_(1.0)
         if self._fallback is not None:
             for gsrc, gdst in zip(self.param_groups, self._fallback.param_groups):
                 gdst["lr"] = gsrc["lr"]
@@ -217,7 +256,8 @@ def get_optimizer_and_param_scheduler(model, args):
     (:152-165) -- and, as in the reference, a missing file is an error, not a silent fresh start."""
     if getattr(args, "fused_optimizer", False):
         optimizer = FusedShardedAdamW(model, lr=args.lr, betas=(getattr(args, "adam_beta1", 0.9), getattr(args, "adam_beta2", 0.999)),
-                                      eps=getattr(args, "adam_eps", 1e-8), weight_decay=args.adam_weight_decay)
+                                      eps=getattr(args, "adam_eps", 1e-8), weight_decay=args.adam_weight_decay,
+                                      clip_grad=float(getattr(args, "clip_grad", 0.0) or 0.0))
     else:
         params = list(model.parameters())
         optimizer = torch.optim.AdamW(params, lr=args.lr, weight_decay=args.adam_weight_decay,
@@ -257,6 +297,27 @@ def _tp_replicated_ranges(unit):
     return [(off, n) for p, off, n in zip(unit.params, unit.offsets, unit.numels) if not getattr(p, "tensor_model_parallel", False)]
 
 
+def _shard_skip_ranges(unit, rank):
+    """Shard-relative [lo, hi) element ranges of a fused unit's gradient that this rank must leave out of the global norm: the
+    tensor-parallel duplicates (``_tp_replicated_ranges``) on tensor-parallel ranks other than 0, rounded out to the 8-element
+    parameter alignment (the padding between parameters holds zero gradients) and merged where they touch."""
+    tp = unit.tp_group
+    if tp is None or tp.size == 1 or tp.rank_in_group(rank) == 0:
+        return []
+    lo = unit.rank_in_group * unit.shard_elems         # this rank's window of the flat buffer
+    hi = lo + unit.shard_elems
+    out = []
+    for off, n in _tp_replicated_ranges(unit):
+        a, b = max(off, lo), min((off + n + 7) // 8 * 8, hi)
+        if a >= b:
+            continue
+        if out and out[-1][1] == a - lo:
+            out[-1] = (out[-1][0], b - lo)
+        else:
+            out.append((a - lo, b - lo))
+    return out
+
+
 def clip_grad_norm(model, max_norm, norm_type=2):
     """Global L2 norm of the gradients over the job, then scale them by min(1, max_norm / (norm + 1e-6))
     (utils.py:124-133 -> megatron ``clip_grad_norm_fp32``, clip_grads.py:47-132).  Every parameter is counted exactly once:
@@ -265,17 +326,24 @@ def clip_grad_norm(model, max_norm, norm_type=2):
       * tensor-parallel ranks hold different slices of the parallel weights, but the SAME norm weights / row-parallel bias
         (after the sequence-parallel gradient all-reduce): those are counted on tensor-parallel rank 0 only.
     Every rank enters the world all-reduce, whether or not it holds gradients.  With ``--fused_optimizer`` the gradient is consumed
-    inside the reduce-scatter kernel and there is nothing left to clip: that combination is rejected."""
+    inside the reduce-scatter kernel and there is nothing left to clip, unless the optimizer was built with ``clip_grad`` > 0: the
+    fused units' squares then come from the norm passes, and the coefficient is stored on the device for ``step()`` (a second
+    call multiplies it, as scaling the gradients twice does)."""
     from .backend import get_backend
     if norm_type != 2:
         raise ValueError("clip_grad_norm: only the L2 norm is implemented")
     be = get_backend()
     units = list(model.model.units)
-    if any(u.uses_fused_optimizer() for u in units):
-        raise RuntimeError("clip_grad_norm cannot be combined with --fused_optimizer: the AdamW step runs inside the gradient "
-                           "reduce-scatter kernel, no gradient tensor survives it (use the unfused optimizer to clip)")
+    fused = next((u.fused_opt for u in units if u.uses_fused_optimizer()), None)
+    if fused is not None and not fused.deferred:
+        raise RuntimeError("clip_grad_norm cannot be combined with --fused_optimizer unless clip_grad > 0: the AdamW step runs inside "
+                           "the gradient reduce-scatter kernel, no gradient tensor survives it (set args.clip_grad to defer the "
+                           "update until the norm is known, or use the unfused optimizer to clip)")
     device = units[0].flat_param.device if units else be.device
     total = torch.zeros((), dtype=torch.float32, device=device)
+    if fused is not None:
+        be.finish_reductions()          # the norm passes have written their partial sums
+        total = total + fused.sum_of_squares()
     grads = []
     for u in units:
         g = u.flat_param.grad
@@ -306,4 +374,6 @@ def clip_grad_norm(model, max_norm, norm_type=2):
     coef = (max_norm / (norm + 1e-6)).clamp(max=1.0)
     for g in grads:
         g.mul_(coef.to(g.dtype))
+    if fused is not None:
+        fused.clip_coef.mul_(coef)
     return float(norm)

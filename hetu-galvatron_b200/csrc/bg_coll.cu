@@ -177,17 +177,44 @@ struct AdamArgs {
     float lr, beta1, beta2, eps, weight_decay, bias_corr1, bias_corr2_sqrt;
 };
 struct RsOut {
-    void* dst;                    // kEpi 0: fp32 shard, 1: bf16 shard, 2: fp32 parameter shard (AdamW)
+    void* dst;                    // kEpi 0: fp32 shard, 1: bf16 shard, 2 / 4: fp32 parameter shard (AdamW), 3: fp32 shard or null
     float* exp_avg;
     float* exp_avg_sq;
     int accumulate;
     AdamArgs a;
+    const float* clip_coef;       // kEpiAdamWClip: the gradient is (sum prescale * x) * (postscale * *clip_coef); null: 1
+    // kEpiSumSq: one fp32 sum of squares of the reduced gradient per warp, in warp order; the entries from 4 * gridDim.x up to
+    // n_partials are zeroed.  Shard-relative element ranges [skip_lo, skip_hi) are left out of the sum.
+    float* partials;
+    int n_partials, n_skip;
+    unsigned long long skip_lo[BG_MAX_SKIP], skip_hi[BG_MAX_SKIP];
 };
-enum { kEpiF32 = 0, kEpiBf16 = 1, kEpiAdamW = 2 };
+// kEpiAdamWClip is kEpiAdamW with the clip coefficient folded into postscale at kernel start: its own instances, so the code of
+// the unclipped ones (and their register allocation) stays as it is
+enum { kEpiF32 = 0, kEpiBf16 = 1, kEpiAdamW = 2, kEpiSumSq = 3, kEpiAdamWClip = 4 };
+constexpr int kWarps = kThreads / 32;
 
 template <int E, int kEpi>
-__device__ __forceinline__ void rs_epilogue(const RsOut& o, size_t v, float* acc, float postscale) {
-    if (kEpi == kEpiBf16) {
+__device__ __forceinline__ void rs_epilogue(const RsOut& o, size_t v, float* acc, float postscale, double& sq) {
+    if (kEpi == kEpiSumSq) {
+        // the norm pass: squares accumulate in fp64 (a thread's sum runs over thousands of elements).  Range bounds are multiples
+        // of 8 elements, so a vector is either inside a skip range or outside all of them.  With a destination the reduced shard
+        // is written as well, with the bits of kEpiF32 (accumulate 0).
+#pragma unroll
+        for (int i = 0; i < E; ++i) acc[i] *= postscale;
+        const unsigned long long e = (unsigned long long)v * E;
+        bool skip = false;
+        for (int r = 0; r < o.n_skip; ++r) skip |= e >= o.skip_lo[r] && e < o.skip_hi[r];
+        if (!skip) {
+#pragma unroll
+            for (int i = 0; i < E; ++i) sq = fma((double)acc[i], (double)acc[i], sq);
+        }
+        if (o.dst != nullptr) {
+            float4* d = reinterpret_cast<float4*>(o.dst) + v * (E / 4);
+#pragma unroll
+            for (int q = 0; q < E / 4; ++q) d[q] = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
+        }
+    } else if (kEpi == kEpiBf16) {
 #pragma unroll
         for (int i = 0; i < E; ++i) acc[i] *= postscale;
         uint4* d = reinterpret_cast<uint4*>(o.dst) + v;
@@ -240,9 +267,11 @@ __device__ __forceinline__ void rs_epilogue(const RsOut& o, size_t v, float* acc
 // multimem.ld_reduce per vector returns the members' sum (fp32 accumulation in the switch, rounded to the source dtype).
 template <int PMAX, int kEpi>
 struct RsPlan {
-    // (the AdamW epilogue keeps 12 more registers of optimizer state live: half the vectors in flight below 8 peers)
-    static constexpr int V = (kEpi == kEpiAdamW && PMAX < 8 ? kInFlight / 2 : kInFlight) / PMAX;
-    static constexpr int V_MC = kEpi == kEpiAdamW ? 4 : 8;
+    // (the AdamW epilogue keeps 12 more registers of optimizer state live, the sum-of-squares epilogue its fp64 sum and the skip
+    // test: half the vectors in flight below 8 peers)
+    static constexpr bool kHalf = kEpi == kEpiAdamW || kEpi == kEpiAdamWClip || kEpi == kEpiSumSq;
+    static constexpr int V = (kHalf && PMAX < 8 ? kInFlight / 2 : kInFlight) / PMAX;
+    static constexpr int V_MC = kHalf ? 4 : 8;
 };
 
 template <int PMAX, bool kSrcBf16, int kEpi, bool kMc>
@@ -255,6 +284,8 @@ __global__ void BG_SLIM reduce_scatter_pull_kernel(const __grid_constant__ PeerP
     const size_t nvec = shard_elems / E;
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     const size_t slice_off = (size_t)s.me * shard_elems * (kSrcBf16 ? 2 : 4);
+    if (kEpi == kEpiAdamWClip && o.clip_coef != nullptr) postscale *= *o.clip_coef;
+    double sq = 0.0;
     for (size_t v0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x; v0 < nvec; v0 += stride * V) {
         uint4 in[V][NL];
         // issue every load of this iteration before consuming any
@@ -286,10 +317,29 @@ __global__ void BG_SLIM reduce_scatter_pull_kernel(const __grid_constant__ PeerP
 #pragma unroll
             for (int k = 0; k < NL; ++k)
                 if (kMc || k < s.n) rs_accumulate<kSrcBf16>(in[u][k], acc, prescale);
-            rs_epilogue<E, kEpi>(o, v, acc, postscale);
+            rs_epilogue<E, kEpi>(o, v, acc, postscale, sq);
         }
     }
+    if (kEpi == kEpiSumSq) {        // warp sums in a fixed order, one entry per warp, the rest of the slot zeroed
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, off);
+        if ((threadIdx.x & 31) == 0) o.partials[blockIdx.x * kWarps + threadIdx.x / 32] = (float)sq;
+        if (blockIdx.x == 0)
+            for (int i = gridDim.x * kWarps + threadIdx.x; i < o.n_partials; i += blockDim.x) o.partials[i] = 0.f;
+    }
     sync_peers<true, false, false>(s);  // every member has finished reading my src: it may be overwritten
+}
+
+// The clipped AdamW step on a local fp32 gradient (pooled ZeRO-3 units keep theirs in an fp32 shard until the step): the
+// epilogue of the reduce-scatter above, with the gradient loaded instead of reduced.
+__global__ void BG_SLIM adamw_local_kernel(const float* __restrict__ grad, const __grid_constant__ RsOut o, size_t n) {
+    const float coef = o.clip_coef != nullptr ? *o.clip_coef : 1.f;
+    double unused = 0.0;
+    for (size_t v = (size_t)blockIdx.x * blockDim.x + threadIdx.x; v < n / 4; v += (size_t)gridDim.x * blockDim.x) {
+        const float4 g = reinterpret_cast<const float4*>(grad)[v];
+        float acc[4] = {g.x, g.y, g.z, g.w};
+        rs_epilogue<4, kEpiAdamW>(o, v, acc, coef, unused);
+    }
 }
 
 template <bool kSrcBf16, int kEpi>
@@ -669,6 +719,23 @@ int bg_preload_coll() {
         K((reduce_scatter_pull_kernel<4, false, kEpiAdamW, false>)),
         K((reduce_scatter_pull_kernel<8, false, kEpiAdamW, false>)),
         K((reduce_scatter_pull_kernel<2, false, kEpiAdamW, true>)),
+        K((reduce_scatter_pull_kernel<2, true, kEpiSumSq, false>)),
+        K((reduce_scatter_pull_kernel<4, true, kEpiSumSq, false>)),
+        K((reduce_scatter_pull_kernel<8, true, kEpiSumSq, false>)),
+        K((reduce_scatter_pull_kernel<2, true, kEpiSumSq, true>)),
+        K((reduce_scatter_pull_kernel<2, false, kEpiSumSq, false>)),
+        K((reduce_scatter_pull_kernel<4, false, kEpiSumSq, false>)),
+        K((reduce_scatter_pull_kernel<8, false, kEpiSumSq, false>)),
+        K((reduce_scatter_pull_kernel<2, false, kEpiSumSq, true>)),
+        K((reduce_scatter_pull_kernel<2, true, kEpiAdamWClip, false>)),
+        K((reduce_scatter_pull_kernel<4, true, kEpiAdamWClip, false>)),
+        K((reduce_scatter_pull_kernel<8, true, kEpiAdamWClip, false>)),
+        K((reduce_scatter_pull_kernel<2, true, kEpiAdamWClip, true>)),
+        K((reduce_scatter_pull_kernel<2, false, kEpiAdamWClip, false>)),
+        K((reduce_scatter_pull_kernel<4, false, kEpiAdamWClip, false>)),
+        K((reduce_scatter_pull_kernel<8, false, kEpiAdamWClip, false>)),
+        K((reduce_scatter_pull_kernel<2, false, kEpiAdamWClip, true>)),
+        K(adamw_local_kernel),
         K((all_reduce_oneshot_kernel<2, true, true>)),
         K((all_reduce_oneshot_kernel<2, true, false>)),
         K((all_reduce_oneshot_kernel<2, false, true>)),
@@ -760,18 +827,26 @@ static int launch_reduce_scatter(bg_ctx_t c, int gid, int lane, const size_t* sr
     BG_CUDA(cudaSetDevice(c->device));
     const char* mc = g_tun.nvls_reduce ? mc_ptr(c, gid, *g, src_offs, shard_elems * g->n * ssz) : nullptr;
     if (mc && shard_elems * ssz < (size_t)g_tun.nvls_min_bytes) mc = nullptr;
-    const bool adam = epi == kEpiAdamW;
+    const bool half = epi == kEpiAdamW || epi == kEpiAdamWClip || epi == kEpiSumSq;
     const int pmax = g->n <= 2 ? 2 : g->n <= 4 ? 4 : 8;
-    const int in_flight_vecs = mc ? (adam ? 4 : 8) : (adam && pmax < 8 ? kInFlight / 2 : kInFlight) / pmax;
+    const int in_flight_vecs = mc ? (half ? 4 : 8) : (half && pmax < 8 ? kInFlight / 2 : kInFlight) / pmax;
     int grid = comm_grid(shard_elems / per / in_flight_vecs + 1, kThreads, g->n);
+    if (o.partials != nullptr && (long long)grid * kWarps > o.n_partials)
+        return fail(BG_EINVAL, "sum-of-squares partials: %d entries, the launch needs %d", o.n_partials, grid * kWarps);
     cudaStream_t st = (cudaStream_t)stream;
     const bool bf = src_dtype == BG_BF16;
-    if (bf && epi == kEpiF32) launch_rs<true, kEpiF32>(g->n, mc != nullptr, grid, st, src, mc, o, shard_elems, prescale, postscale, s);
-    else if (bf && epi == kEpiBf16) launch_rs<true, kEpiBf16>(g->n, mc != nullptr, grid, st, src, mc, o, shard_elems, prescale, postscale, s);
-    else if (bf && epi == kEpiAdamW) launch_rs<true, kEpiAdamW>(g->n, mc != nullptr, grid, st, src, mc, o, shard_elems, prescale, postscale, s);
-    else if (!bf && epi == kEpiF32) launch_rs<false, kEpiF32>(g->n, mc != nullptr, grid, st, src, mc, o, shard_elems, prescale, postscale, s);
-    else if (!bf && epi == kEpiAdamW) launch_rs<false, kEpiAdamW>(g->n, mc != nullptr, grid, st, src, mc, o, shard_elems, prescale, postscale, s);
+#define BG_RS_EPI(B, E) launch_rs<B, E>(g->n, mc != nullptr, grid, st, src, mc, o, shard_elems, prescale, postscale, s)
+    if (bf && epi == kEpiF32) BG_RS_EPI(true, kEpiF32);
+    else if (bf && epi == kEpiBf16) BG_RS_EPI(true, kEpiBf16);
+    else if (bf && epi == kEpiAdamW) BG_RS_EPI(true, kEpiAdamW);
+    else if (bf && epi == kEpiSumSq) BG_RS_EPI(true, kEpiSumSq);
+    else if (bf && epi == kEpiAdamWClip) BG_RS_EPI(true, kEpiAdamWClip);
+    else if (!bf && epi == kEpiF32) BG_RS_EPI(false, kEpiF32);
+    else if (!bf && epi == kEpiAdamW) BG_RS_EPI(false, kEpiAdamW);
+    else if (!bf && epi == kEpiSumSq) BG_RS_EPI(false, kEpiSumSq);
+    else if (!bf && epi == kEpiAdamWClip) BG_RS_EPI(false, kEpiAdamWClip);
     else return fail(BG_EUNSUPPORTED, "reduce_scatter %d -> epilogue %d", src_dtype, epi);
+#undef BG_RS_EPI
     BG_CHECK_LAUNCH();
     return BG_OK;
 }
@@ -787,18 +862,66 @@ extern "C" int bg_reduce_scatter_acc(bg_ctx_t c, int gid, int lane, const size_t
                                  postscale, stream);
 }
 
+static int adam_out(float* param, float* exp_avg, float* exp_avg_sq, float lr, float beta1, float beta2, float eps,
+                    float weight_decay, long long step, RsOut* o) {
+    if (((uintptr_t)param | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) % 16) return fail(BG_EINVAL, "optimizer state not 16-B aligned");
+    if (step < 1) return fail(BG_EINVAL, "adam step must be >= 1");
+    o->dst = param; o->exp_avg = exp_avg; o->exp_avg_sq = exp_avg_sq;
+    o->a.lr = lr; o->a.beta1 = beta1; o->a.beta2 = beta2; o->a.eps = eps; o->a.weight_decay = weight_decay;
+    o->a.bias_corr1 = (float)(1.0 - pow((double)beta1, (double)step));
+    o->a.bias_corr2_sqrt = (float)sqrt(1.0 - pow((double)beta2, (double)step));
+    return BG_OK;
+}
+
 extern "C" int bg_reduce_scatter_adamw(bg_ctx_t c, int gid, int lane, const size_t* src_offs, int src_dtype, float* param,
                                        float* exp_avg, float* exp_avg_sq, size_t shard_elems, float prescale, float postscale,
                                        float lr, float beta1, float beta2, float eps, float weight_decay, long long step,
                                        void* stream) {
-    if (((uintptr_t)param | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) % 16) return fail(BG_EINVAL, "optimizer state not 16-B aligned");
-    if (step < 1) return fail(BG_EINVAL, "adam step must be >= 1");
     RsOut o = {};
-    o.dst = param; o.exp_avg = exp_avg; o.exp_avg_sq = exp_avg_sq;
-    o.a.lr = lr; o.a.beta1 = beta1; o.a.beta2 = beta2; o.a.eps = eps; o.a.weight_decay = weight_decay;
-    o.a.bias_corr1 = (float)(1.0 - pow((double)beta1, (double)step));
-    o.a.bias_corr2_sqrt = (float)sqrt(1.0 - pow((double)beta2, (double)step));
+    int rc = adam_out(param, exp_avg, exp_avg_sq, lr, beta1, beta2, eps, weight_decay, step, &o);
+    if (rc) return rc;
     return launch_reduce_scatter(c, gid, lane, src_offs, src_dtype, kEpiAdamW, o, shard_elems, prescale, postscale, stream);
+}
+
+extern "C" int bg_reduce_scatter_adamw_clipped(bg_ctx_t c, int gid, int lane, const size_t* src_offs, int src_dtype, float* param,
+                                               float* exp_avg, float* exp_avg_sq, size_t shard_elems, float prescale,
+                                               float postscale, float lr, float beta1, float beta2, float eps, float weight_decay,
+                                               long long step, const float* clip_coef, void* stream) {
+    RsOut o = {};
+    int rc = adam_out(param, exp_avg, exp_avg_sq, lr, beta1, beta2, eps, weight_decay, step, &o);
+    if (rc) return rc;
+    o.clip_coef = clip_coef;
+    return launch_reduce_scatter(c, gid, lane, src_offs, src_dtype, kEpiAdamWClip, o, shard_elems, prescale, postscale, stream);
+}
+
+extern "C" int bg_reduce_scatter_sumsq(bg_ctx_t c, int gid, int lane, const size_t* src_offs, int src_dtype, float* dst,
+                                       size_t shard_elems, float prescale, float postscale, float* partials, int n_partials,
+                                       const size_t* skip, int n_skip, void* stream) {
+    if (partials == nullptr || n_partials < 1) return fail(BG_EINVAL, "sum-of-squares partials missing");
+    if (n_skip < 0 || n_skip > BG_MAX_SKIP) return fail(BG_EINVAL, "%d skip ranges (at most %d)", n_skip, BG_MAX_SKIP);
+    RsOut o = {};
+    o.dst = dst; o.partials = partials; o.n_partials = n_partials; o.n_skip = n_skip;
+    for (int r = 0; r < n_skip; ++r) {
+        if (skip[2 * r] % 8 || skip[2 * r + 1] % 8 || skip[2 * r] > skip[2 * r + 1])
+            return fail(BG_EINVAL, "skip range [%zu, %zu) is not 8-element aligned", skip[2 * r], skip[2 * r + 1]);
+        o.skip_lo[r] = skip[2 * r]; o.skip_hi[r] = skip[2 * r + 1];
+    }
+    if (dst != nullptr && (uintptr_t)dst % 16) return fail(BG_EINVAL, "dst not 16-B aligned");
+    return launch_reduce_scatter(c, gid, lane, src_offs, src_dtype, kEpiSumSq, o, shard_elems, prescale, postscale, stream);
+}
+
+extern "C" int bg_adamw_clipped(float* param, float* exp_avg, float* exp_avg_sq, const float* grad, size_t n, float lr, float beta1,
+                                float beta2, float eps, float weight_decay, long long step, const float* clip_coef, void* stream) {
+    RsOut o = {};
+    int rc = adam_out(param, exp_avg, exp_avg_sq, lr, beta1, beta2, eps, weight_decay, step, &o);
+    if (rc) return rc;
+    if (n % 4 || (uintptr_t)grad % 16) return fail(BG_EINVAL, "adamw: %zu elements / gradient alignment (need multiples of 4, 16 B)", n);
+    if (n == 0) return BG_OK;
+    o.clip_coef = clip_coef;
+    const int grid = comm_grid(n / 4, kThreads, 1);
+    adamw_local_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(grad, o, n);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
 }
 
 extern "C" int bg_all_reduce(bg_ctx_t c, int gid, int lane, const size_t* src_offs, void* dst, size_t elems, int dtype,

@@ -122,6 +122,30 @@ int bg_reduce_scatter_adamw(bg_ctx_t ctx, int gid, int lane, const size_t* src_o
                             float* exp_avg_sq, size_t shard_elems, float prescale, float postscale, float lr, float beta1,
                             float beta2, float eps, float weight_decay, long long step, void* stream);
 
+/* Gradient clipping by the global norm with the fused optimizer, in two passes over the same unsharded gradient.
+ * Norm pass: the pull reduce-scatter above forms the reduced fp32 value (sum prescale * x) * postscale and writes, per warp of the
+ * launch, the fp32 sum of its squares into `partials` (warp order; the entries past the launch's 4 * grid are zeroed; BG_EINVAL
+ * when `n_partials` is too small -- 4 x comm_ctas, or 4 x local_ctas for a group of one, always suffice).  The sums accumulate in
+ * fp64 in a fixed order: no atomics, run-to-run deterministic.  `skip` holds `n_skip` (<= BG_MAX_SKIP) shard-relative element
+ * ranges [lo, hi), multiples of 8, left out of the sum (tensor-parallel duplicates).  `dst` null: nothing else is written; non-null:
+ * also the fp32 shard, bit-identical to bg_reduce_scatter_acc's (accumulate 0). */
+#define BG_MAX_SKIP 16
+int bg_reduce_scatter_sumsq(bg_ctx_t ctx, int gid, int lane, const size_t* src_offs, int src_dtype, float* dst, size_t shard_elems,
+                            float prescale, float postscale, float* partials, int n_partials, const size_t* skip, int n_skip,
+                            void* stream);
+
+/* Step pass: bg_reduce_scatter_adamw with the reduced gradient multiplied by the device scalar *clip_coef (null: 1) before the
+ * moments are updated.  At a coefficient of 1 the result is bit-identical to bg_reduce_scatter_adamw's. */
+int bg_reduce_scatter_adamw_clipped(bg_ctx_t ctx, int gid, int lane, const size_t* src_offs, int src_dtype, float* param,
+                                    float* exp_avg, float* exp_avg_sq, size_t shard_elems, float prescale, float postscale, float lr,
+                                    float beta1, float beta2, float eps, float weight_decay, long long step, const float* clip_coef,
+                                    void* stream);
+
+/* The same clipped AdamW rule on a local fp32 gradient `grad` of n elements (a multiple of 4): the step of units whose gradient
+ * was reduced into an fp32 shard by the norm pass. */
+int bg_adamw_clipped(float* param, float* exp_avg, float* exp_avg_sq, const float* grad, size_t n, float lr, float beta1,
+                     float beta2, float eps, float weight_decay, long long step, const float* clip_coef, void* stream);
+
 /* C3/C5/C6/C13/C14/C16  all-reduce (sum|max), out of place: src is a symmetric buffer, dst any local pointer.
  * Replaces _runtime_utils.py:940 (DDP grads), mappings_group.py:19 _reduce (row-parallel fwd, layers.py:1114;
  * column-parallel bwd, mappings_group.py:139), cross_entropy.py:22-30,61-72,78-89, grad_reduce.py:121-124.

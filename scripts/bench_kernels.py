@@ -1,5 +1,5 @@
 """Micro-benchmarks of the C-ABI kernels on one GPU (CUDA events, warm-up, L2-exceeding inputs).
-Usage: python scripts/bench_kernels.py [gemm] [cast] [ops] [attn] [dropout] [cp]  -> JSON lines on stdout."""
+Usage: python scripts/bench_kernels.py [gemm] [cast] [ops] [attn] [dropout] [cp] [clip]  -> JSON lines on stdout."""
 import json
 import os
 import sys
@@ -398,6 +398,55 @@ def cp():
             del k, v, dk, dv
             torch.cuda.empty_cache()
     be.close()
+
+
+def clip():
+    """Gradient clipping with the fused optimizer at the flagship units' shard sizes (Llama-3.2-1B, one GPU, p = 1): the norm pass,
+    the clipped step pass and today's unclipped AdamW reduce-scatter, beside what the torch optimizer runs after the backward to
+    clip (pow().sum(), mul_, fused AdamW over the fp32 gradient shard).  GB/s over the algorithmic bytes: norm pass P*gsz, step pass
+    P*gsz + 24*P (read and write param, exp_avg, exp_avg_sq), pow-sum 4P, mul_ 8P, torch fused AdamW 28P."""
+    import subprocess
+    from hetu_galvatron_b200.core.runtime.comm_groups import CommGroup
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    print(json.dumps({"nvidia_smi": q.stdout.strip()}), flush=True)
+    hyper = (1e-4, 0.9, 0.95, 1e-8, 0.01)
+    for unit, P in (("decoder_layer", 60_821_504), ("embed_or_head", 262_668_288)):
+        comm = bg.BgComm(0, 1, 0, P * 2 + (1 << 24))
+        grp = CommGroup([0])
+        g = comm.sym_alloc(grp, P * 2)
+        comm.exchange()
+        g.view(BF, P).copy_(torch.randn(P, device="cuda").to(BF) * 1e-3)
+        p, m, v = torch.randn(P, device="cuda"), torch.zeros(P, device="cuda"), torch.zeros(P, device="cuda")
+        parts = torch.zeros(4 * max(bg.get_tunable("comm_ctas"), bg.get_tunable("local_ctas")), device="cuda")
+        coef = torch.full((), 0.5, device="cuda")
+        runs = {
+            "norm_pass": (lambda: comm.reduce_scatter_sumsq(grp, g, BF, P, 1.0, 1.0, parts), 2 * P),
+            "step_pass_clipped": (lambda: comm.reduce_scatter_adamw_clipped(grp, g, BF, p, m, v, P, 1.0, 1.0, *hyper, 1, coef), 26 * P),
+            "reduce_scatter_adamw": (lambda: comm.reduce_scatter_adamw(grp, g, BF, p, m, v, P, 1.0, 1.0, *hyper, 1), 26 * P),
+        }
+        for name, (fn, nbytes) in runs.items():
+            t = timeit(fn)
+            print(json.dumps({"bench": "clip_" + name, "unit": unit, "elems": P, "ms": round(t, 4),
+                              "GBps_algorithmic": round(nbytes / t / 1e6, 1)}), flush=True)
+        comm.close()
+        del g
+        grad = torch.randn(P, device="cuda") * 1e-3
+        step = torch.ones((), device="cuda")
+        torch_runs = {
+            "torch_pow_sum": (lambda: grad.pow(2).sum(), 4 * P),
+            "torch_mul": (lambda: grad.mul_(coef), 8 * P),
+            "torch_fused_adamw": (lambda: torch._fused_adamw_([p], [grad], [m], [v], [], [step], lr=hyper[0], beta1=hyper[1], beta2=hyper[2],
+                                                              weight_decay=hyper[4], eps=hyper[3], amsgrad=False, maximize=False), 28 * P),
+        }
+        total = 0.0
+        for name, (fn, nbytes) in torch_runs.items():
+            t = timeit(fn)
+            total += t
+            print(json.dumps({"bench": "clip_" + name, "unit": unit, "elems": P, "ms": round(t, 4),
+                              "GBps_algorithmic": round(nbytes / t / 1e6, 1)}), flush=True)
+        print(json.dumps({"bench": "clip_torch_tail_total", "unit": unit, "ms": round(total, 4)}), flush=True)
+        del p, m, v, grad
+        torch.cuda.empty_cache()
 
 
 if __name__ == "__main__":
