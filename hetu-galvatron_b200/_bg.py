@@ -491,7 +491,8 @@ class BgComm:
         (its 256-thread / 128-register kernels could not share an SM, and two of them in flight on different streams could
         deadlock across ranks -- seen with ZeRO-3's concurrent all-gather and reduce-scatter at Llama-70B sizes).  The slim
         kernels (128 threads x <= 64 registers, one CTA per SM, no shared memory) are always co-resident, beside each other
-        and beside a GEMM, so no ordering is imposed any more: collectives on different streams really overlap.
+        and beside a fused GEMM (three of them; two beside a plain GEMM's wider tile, which waits on no peer and always
+        retires), so no ordering is imposed any more: collectives on different streams really overlap.
         ``HGB_SERIAL_COLLECTIVES=1`` restores the chain (debugging aid)."""
         import torch
         s = torch.cuda.current_stream() if stream is None else stream

@@ -1,10 +1,12 @@
 // bg_coll.cu -- the peer-memory collectives (SURVEY 2.3 rows C1-C3, C5-C10, C12-C14, C16) as SLIM kernels.
 //
 // Every cross-rank kernel here is 128 threads x <= 64 registers with no shared memory (8,192 registers per CTA), launched with
-// at most one CTA per SM ("comm_ctas", default 132).  The persistent wgmma GEMM CTA takes 36,864 registers and 193 KiB of the
-// shared memory of its SM, so up to three collectives (e.g. ZeRO-3's prefetch all-gather, the gradient reduce-scatter and a
-// tensor-parallel exchange) are resident BESIDE a running GEMM, and beside each other: a collective never has to wait for a
-// different kernel of its own rank to leave the SMs before its peers can see it arrive.  That removes the cross-rank deadlock
+// at most one CTA per SM ("comm_ctas", default 132).  A 128-wide wgmma GEMM CTA (every fused GEMM, and plain GEMMs of N <= 128)
+// takes 36,864 registers and 193 KiB of the shared memory of its SM, so up to three collectives (e.g. ZeRO-3's prefetch
+// all-gather, the gradient reduce-scatter and a tensor-parallel exchange) are resident BESIDE it, and beside each other: a
+// collective never has to wait for a different kernel of its own rank to leave the SMs before its peers can see it arrive.
+// A 256-wide plain GEMM CTA (48,384 registers, 209 KiB) leaves room for two; a third waits at most until that GEMM, which
+// waits on nothing, retires (bg_gemm.cu, DESIGN section 2).  That removes the cross-rank deadlock
 // of round 1's 256-thread / 128-register kernels (two of them could not share an SM; rank A ran the all-gather and rank B the
 // reduce-scatter, each waiting for the peer kernel that could not become resident) without serialising the collectives on the
 // host.  Bandwidth: a peer load takes ~2,000 cycles (~1.8 us) over NVSwitch; 132 x 128 threads x 8 x 16 B = 2.2 MB in

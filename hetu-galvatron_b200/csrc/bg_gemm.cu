@@ -2,15 +2,19 @@
 // by TMA with 128-B swizzle), persistent, warp-specialised.  Replaces the torch.matmul -> cuBLAS calls of
 // galvatron/site_package/megatron/core/tensor_parallel/layers.py:417 (fwd), :462 (dgrad), :534 (wgrad).
 //
-//   tile            : BLOCK_M 128 x BLOCK_N 128 x BLOCK_K 64, one CTA per SM; two consumer warpgroups, each issuing
-//                     wgmma m64n128k16 on its 64 rows of the tile (64 fp32 accumulators per thread)
-//   smem pipeline   : 5 stages x (A 16 KiB + B 16 KiB), full/empty mbarriers (TMA <-> wgmma)
+//   tile            : BLOCK_M 128 x (128 | 256) x BLOCK_K 64, one CTA per SM; two consumer warpgroups, each issuing
+//                     wgmma m64n128k16 (64 fp32 accumulators per thread) or m64n256k16 (128) on its 64 rows of the tile.
+//                     The plain GEMM runs 256-wide tiles for N > 128 (half the shared-memory operand reads per FLOP of
+//                     the 128-wide tile); the fused modes and plain GEMMs of N <= 128 run 128-wide tiles.
+//   smem pipeline   : 128-wide: 5 stages x (A 16 KiB + B 16 KiB); 256-wide: 4 stages x (A 16 KiB + B 32 KiB);
+//                     full/empty mbarriers (TMA <-> wgmma)
 //   warps           : 0-7 = the two consumer warpgroups (wgmma, then the epilogue: registers -> swizzled smem -> TMA store),
 //                     8 = TMA producer; 288 threads.  The producer fills the stages of the next tile while the consumers run
 //                     the epilogue of this one.
-//   residency       : <= 136 registers per thread (288 x 136 = 39,168 per CTA) and 193 KiB of shared memory, so three slim
-//                     collective CTAs (128 threads x 64 registers, no shared memory, bg_coll.cu) stay resident beside a
-//                     running GEMM CTA
+//   residency       : slim collective CTAs (128 threads x 64 registers, no shared memory, bg_coll.cu) stay resident beside
+//                     a running GEMM CTA: three beside a 128-wide CTA (<= 136 registers per thread, 193 KiB of shared
+//                     memory), which every kernel that waits on peers needs; two beside a 256-wide plain CTA (<= 168
+//                     registers, 209 KiB), which waits on nothing and always retires (DESIGN section 2)
 //   layouts         : TN  C = A[M,K] * B[N,K]^T   (A, B K-major)
 //                     NN  C = A[M,K] * B[K,N]     (B MN-major: TMA boxes of 64 N-elements x 64 K-rows)
 //                     NT  C = A[K,M]^T * B[K,N]   (A, B MN-major)
@@ -23,22 +27,37 @@ using namespace bg;
 
 namespace {
 
-constexpr int BLOCK_M = 128, BLOCK_N = 128, BLOCK_K = 64, WGMMA_K = 16;
-constexpr int kStages = 5;
-constexpr int kABytes = BLOCK_M * BLOCK_K * 2, kBBytes = BLOCK_N * BLOCK_K * 2, kStageBytes = kABytes + kBBytes;
+constexpr int BLOCK_M = 128, BLOCK_N = 128, BLOCK_K = 64, WGMMA_K = 16;   // BLOCK_N: the fused modes' tile width
+constexpr int WIDE_N = 256;                                    // the plain GEMM's tile width for N > BLOCK_N
+constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
 constexpr int kStoreCols = 64;                                 // columns per TMA store box (128 B)
 constexpr int kStoreBytes = BLOCK_M * kStoreCols * 2;          // 16 KiB per staging buffer
-constexpr int kNumStoreBufs = 2;
-constexpr int kSmemBytes = kStages * kStageBytes + kNumStoreBufs * kStoreBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 constexpr int kEpiThreads = 256, kThreads = kEpiThreads + 32;  // two consumer warpgroups + one producer warp
 constexpr int kProducerWarp = kEpiThreads / 32;
-constexpr int kMaxRegs = 136;
 constexpr int kWgOffset = 8192;  // smem offset of consumer warpgroup 1's operand A: 64 K-major rows, or the 2nd 64-wide M chunk
 constexpr int kGroupM = 16;      // tile raster of the fused modes: 16 m-blocks share each sweep over n (L2 reuse)
-static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KiB of shared memory per block");
-static_assert(kThreads * kMaxRegs + 3 * 128 * 64 <= 65536, "a GEMM CTA and three slim collective CTAs share an SM's registers");
-// H100: 228 KiB of shared memory per SM, of which the driver reserves 1 KiB per resident CTA (also for a CTA that uses none)
-static_assert(kSmemBytes + 1024 + 3 * 1024 <= 228 * 1024, "a GEMM CTA and three slim collective CTAs share an SM's shared memory");
+
+// Pipeline and residency of one tile width.  A kernel that waits on peers (the fused modes, every collective) must always be
+// resident beside one CTA of each other collective that can be in flight: a 128-wide GEMM CTA leaves room for three slim
+// CTAs.  A 256-wide plain GEMM CTA leaves room for two: it waits on nothing after launch, so a third collective CTA that
+// cannot become resident beside it waits at most until it retires, and no cycle of waits passes through it.
+template <int kBlockN>
+struct Tile {
+    static constexpr bool kWide = kBlockN == WIDE_N;
+    static constexpr int kStages = kWide ? 4 : 5;
+    static constexpr int kNumStoreBufs = kWide ? 1 : 2;
+    static constexpr int kMaxRegs = kWide ? 168 : 136;         // 128 (64) fp32 accumulators per consumer thread
+    static constexpr int kSlimCtas = kWide ? 2 : 3;
+    static constexpr int kBBytes = kBlockN * BLOCK_K * 2, kStageBytes = kABytes + kBBytes;
+    static constexpr int kSmemBytes = kStages * kStageBytes + kNumStoreBufs * kStoreBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+    static_assert(kBlockN == BLOCK_N || kBlockN == WIDE_N, "tile width 128 or 256");
+    static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KiB of shared memory per block");
+    static_assert(kThreads * kMaxRegs + kSlimCtas * 128 * 64 <= 65536, "a GEMM CTA and its slim collective CTAs share an SM's registers");
+    // H100: 228 KiB of shared memory per SM, of which the driver reserves 1 KiB per resident CTA (also for a CTA that uses none)
+    static_assert(kSmemBytes + 1024 + kSlimCtas * 1024 <= 228 * 1024, "a GEMM CTA and its slim collective CTAs share an SM's shared memory");
+};
+template struct Tile<BLOCK_N>;
+template struct Tile<WIDE_N>;
 
 enum Layout { kTN = 0, kNN = 1, kNT = 2 };
 
@@ -89,9 +108,10 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from touching the accumulators across an asynchronous wgmma (register dependences only)
+template <int kNumAcc>
 __device__ __forceinline__ void fence_acc(float* d) {
 #pragma unroll
-    for (int i = 0; i < BLOCK_N / 2; ++i) asm volatile("" : "+f"(d[i])::"memory");
+    for (int i = 0; i < kNumAcc; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // D[64 x 128] (+)= A[64 x 16] * B[16 x 128], both operands in shared memory; kTransA / kTransB = 1 for an MN-major operand
@@ -114,6 +134,41 @@ __device__ __forceinline__ void wgmma_m64n128(float* d, uint64_t desc_a, uint64_
           "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
           "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
           "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(kTransA), "n"(kTransB));
+}
+
+// D[64 x 256] (+)= A[64 x 16] * B[16 x 256]: as above, 128 accumulators per thread
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_m64n256(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+        "%128, %129, p, 1, 1, %131, %132;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
         : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(kTransA), "n"(kTransB));
 }
 
@@ -197,15 +252,18 @@ __device__ __forceinline__ TileCoord tile_of(int t, int m_blocks, int n_blocks, 
     return tc;
 }
 
-template <int kLayout, int kMode = kPlain>
-__global__ void __maxnreg__(kMaxRegs) gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a,
+template <int kLayout, int kMode = kPlain, int kBlockN = BLOCK_N>
+__global__ void __maxnreg__(Tile<kBlockN>::kMaxRegs) gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                 const __grid_constant__ CUtensorMap map_b,
                                                                 const __grid_constant__ CUtensorMap map_c,
                                                                 const __nv_bfloat16* __restrict__ c_old, int M, int N, int K,
                                                                 int accumulate,
                                                                 const __grid_constant__ FuseParams<kMode> sp) {
+    static_assert(kMode == kPlain || kBlockN == BLOCK_N, "the fused modes wait on peers: they keep the three-slim-CTA tile");
     constexpr bool kScatter = kMode == kScatterMode, kGather = kMode == kGatherMode;
     constexpr bool kAMn = kLayout == kNT, kBMn = kLayout != kTN;
+    constexpr int kStages = Tile<kBlockN>::kStages, kStageBytes = Tile<kBlockN>::kStageBytes;
+    constexpr int kNumStoreBufs = Tile<kBlockN>::kNumStoreBufs;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* smem_store = smem + kStages * kStageBytes;
@@ -214,7 +272,7 @@ __global__ void __maxnreg__(kMaxRegs) gemm_bf16_kernel(const __grid_constant__ C
     uint64_t* empty_bar = bars + kStages;            // [kStages]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m_blocks = (M + BLOCK_M - 1) / BLOCK_M, n_blocks = (N + BLOCK_N - 1) / BLOCK_N;
+    const int m_blocks = (M + BLOCK_M - 1) / BLOCK_M, n_blocks = (N + kBlockN - 1) / kBlockN;
     const int num_tiles = m_blocks * n_blocks, k_blocks = (K + BLOCK_K - 1) / BLOCK_K;
 
     // Fused scatter: rank r walks the owners in the order r+1, r+2, ..., r (ring schedule, map_m), so at any moment every owner
@@ -279,11 +337,11 @@ __global__ void __maxnreg__(kMaxRegs) gemm_bf16_kernel(const __grid_constant__ C
                     } else {     // A stored [M][K]: one box of 64 K-elements x 128 rows
                         tma_load_2d(sa, amap, bar, kb * BLOCK_K, a_row);
                     }
-                    if (kBMn) {
+                    if (kBMn) {  // B stored [K][N]: kBlockN/64 boxes of 64 N-elements x 64 K-rows
 #pragma unroll
-                        for (int j = 0; j < BLOCK_N / 64; ++j) tma_load_2d(sb + j * (BLOCK_K * 128), &map_b, bar, tc.n * BLOCK_N + j * 64, kb * BLOCK_K);
-                    } else {
-                        tma_load_2d(sb, &map_b, bar, kb * BLOCK_K, tc.n * BLOCK_N);
+                        for (int j = 0; j < kBlockN / 64; ++j) tma_load_2d(sb + j * (BLOCK_K * 128), &map_b, bar, tc.n * kBlockN + j * 64, kb * BLOCK_K);
+                    } else {     // B stored [N][K]: one box of 64 K-elements x kBlockN rows
+                        tma_load_2d(sb, &map_b, bar, kb * BLOCK_K, tc.n * kBlockN);
                     }
                     if (++stage == kStages) { stage = 0; phase ^= 1; }
                 }
@@ -299,9 +357,9 @@ __global__ void __maxnreg__(kMaxRegs) gemm_bf16_kernel(const __grid_constant__ C
         // MN-major: 64-element MN chunks BLOCK_K*128 B apart (LBO), 8-k-row groups 1024 B apart (SBO), K step 16 rows
         constexpr uint32_t a_lbo = kAMn ? BLOCK_K * 128 : 0, b_lbo = kBMn ? BLOCK_K * 128 : 0;
         constexpr uint32_t a_kstep = kAMn ? WGMMA_K * 128 : WGMMA_K * 2, b_kstep = kBMn ? WGMMA_K * 128 : WGMMA_K * 2;
-        float acc[BLOCK_N / 2];
+        float acc[kBlockN / 2];
 #pragma unroll
-        for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+        for (int i = 0; i < kBlockN / 2; ++i) acc[i] = 0.f;
         int stage = 0; uint32_t phase = 0;
         int buf = 0;
         uint32_t* prev_flag = nullptr;                // fused scatter: arrival counter of the tile whose stores are in flight
@@ -317,7 +375,8 @@ __global__ void __maxnreg__(kMaxRegs) gemm_bf16_kernel(const __grid_constant__ C
                 for (int k = 0; k < BLOCK_K / WGMMA_K; ++k) {
                     const uint64_t da = make_smem_desc(sa + k * a_kstep, a_lbo, 1024);
                     const uint64_t db = make_smem_desc(sb + k * b_kstep, b_lbo, 1024);
-                    wgmma_m64n128<kAMn ? 1 : 0, kBMn ? 1 : 0>(acc, da, db, (kb | k) != 0);
+                    if constexpr (kBlockN == WIDE_N) wgmma_m64n256<kAMn ? 1 : 0, kBMn ? 1 : 0>(acc, da, db, (kb | k) != 0);
+                    else wgmma_m64n128<kAMn ? 1 : 0, kBMn ? 1 : 0>(acc, da, db, (kb | k) != 0);
                 }
                 wgmma_commit();
                 wgmma_wait<1>();                               // k-block kb-1's wgmmas have retired: its stage is free
@@ -326,14 +385,31 @@ __global__ void __maxnreg__(kMaxRegs) gemm_bf16_kernel(const __grid_constant__ C
                 if (++stage == kStages) { stage = 0; phase ^= 1; }
             }
             wgmma_wait<0>();
-            fence_acc(acc);
+            fence_acc<kBlockN / 2>(acc);
             if (lane == 0) mbar_arrive(smem_u32(empty_bar + prev_stage));
 #pragma unroll
-            for (int c = 0; c < BLOCK_N / kStoreCols; ++c) {
-                const int n0 = tc.n * BLOCK_N + c * kStoreCols;
+            for (int c = 0; c < kBlockN / kStoreCols; ++c) {
+                const int n0 = tc.n * kBlockN + c * kStoreCols;
                 if (n0 >= N) break;  // whole chunk out of bounds (uniform across the CTA)
                 float* v = acc + c * (kStoreCols / 2);         // 8 column groups x {row, row + 8} x 2 columns
-                if (accumulate) {
+                if (accumulate && Tile<kBlockN>::kWide) {
+                    // 128 accumulators leave 40 registers: int row bounds and one base pointer per row
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int grow = tc.m * BLOCK_M + frag_row + 8 * h;
+                        if (grow < M) {
+                            const uint32_t* src = reinterpret_cast<const uint32_t*>(c_old + (long long)grow * N + n0 + frag_col);
+#pragma unroll
+                            for (int j = 0; j < 8; ++j) {
+                                if (n0 + j * 8 < N) {
+                                    const float2 o = bf2_to_f2(src[j * 4]);
+                                    v[j * 4 + 2 * h] += o.x;
+                                    v[j * 4 + 2 * h + 1] += o.y;
+                                }
+                            }
+                        }
+                    }
+                } else if (accumulate) {
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const long long grow = (long long)tc.m * BLOCK_M + frag_row + 8 * h;
@@ -349,17 +425,32 @@ __global__ void __maxnreg__(kMaxRegs) gemm_bf16_kernel(const __grid_constant__ C
                         }
                     }
                 }
-                // staging buffer `buf` must be free: the store issued two chunks ago has finished reading it
+                // staging buffer `buf` must be free: the store issued kNumStoreBufs chunks ago has finished reading it
                 if (issuer) tma_store_wait_read<kNumStoreBufs - 1>();
                 epi_bar_sync();
                 uint8_t* sbuf = smem_store + buf * kStoreBytes;
+                if constexpr (Tile<kBlockN>::kWide) {
+                    // The same swizzle as one XOR per store on a single row address (the buffer is 1024-B aligned, so bits 4-6
+                    // of the address are the 16-B chunk).  The empty asm keeps the compiler from hoisting the eight chunk
+                    // addresses out of the tile loop, which would cost eight registers.
+                    uint32_t srow = smem_u32(sbuf) + frag_row * 128 + ((frag_row & 7) << 4) + frag_col * 2;
+                    asm volatile("" : "+r"(srow));
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int row = frag_row + 8 * h;
+                    for (int h = 0; h < 2; ++h) {   // row + 8: 1024 B further, same (row & 7)
 #pragma unroll
-                    for (int j = 0; j < 8; ++j)   // 128-B swizzle: 16-B chunk j of row r lives at chunk (j ^ (r & 7))
-                        *reinterpret_cast<uint32_t*>(sbuf + row * 128 + ((j ^ (row & 7)) << 4) + frag_col * 2) =
-                            f2_to_bf2(v[j * 4 + 2 * h], v[j * 4 + 2 * h + 1]);
+                        for (int j = 0; j < 8; ++j)
+                            asm volatile("st.shared.u32 [%0], %1;" ::"r"((srow + h * 1024) ^ (j << 4)),
+                                         "r"(f2_to_bf2(v[j * 4 + 2 * h], v[j * 4 + 2 * h + 1])) : "memory");
+                    }
+                } else {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = frag_row + 8 * h;
+#pragma unroll
+                        for (int j = 0; j < 8; ++j)   // 128-B swizzle: 16-B chunk j of row r lives at chunk (j ^ (r & 7))
+                            *reinterpret_cast<uint32_t*>(sbuf + row * 128 + ((j ^ (row & 7)) << 4) + frag_col * 2) =
+                                f2_to_bf2(v[j * 4 + 2 * h], v[j * 4 + 2 * h + 1]);
+                    }
                 }
                 fence_proxy_async();
                 epi_bar_sync();
@@ -372,14 +463,14 @@ __global__ void __maxnreg__(kMaxRegs) gemm_bf16_kernel(const __grid_constant__ C
                     }
                     tma_store_commit();
                 }
-                buf ^= 1;
+                if constexpr (kNumStoreBufs > 1) buf ^= 1;
             }
             if constexpr (kScatter) {
                 if (issuer) {
                     // Publish the PREVIOUS tile: every bulk group except this tile's (<= 2 chunks) has completed, so its peer
                     // stores are done -- no stall on this tile's NVLink latency.
                     if (prev_flag != nullptr) {
-                        asm volatile("cp.async.bulk.wait_group %0;" ::"n"(BLOCK_N / kStoreCols) : "memory");
+                        asm volatile("cp.async.bulk.wait_group %0;" ::"n"(kBlockN / kStoreCols) : "memory");
                         __threadfence_system();
                         asm volatile("red.release.sys.global.add.u32 [%0], 1;" ::"l"(prev_flag) : "memory");
                     }
@@ -452,10 +543,13 @@ static int gemm_setup() {
         BG_CUDA(cudaGetDevice(&dev));
         int sms = 0;
         BG_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-#define BG_SMEM(K) BG_CUDA(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes))
-        BG_SMEM(gemm_bf16_kernel<kTN>); BG_SMEM(gemm_bf16_kernel<kNN>); BG_SMEM(gemm_bf16_kernel<kNT>);
-        BG_SMEM((gemm_bf16_kernel<kTN, kScatterMode>)); BG_SMEM((gemm_bf16_kernel<kNN, kScatterMode>)); BG_SMEM((gemm_bf16_kernel<kNT, kScatterMode>));
-        BG_SMEM((gemm_bf16_kernel<kTN, kGatherMode>)); BG_SMEM((gemm_bf16_kernel<kNN, kGatherMode>));
+#define BG_SMEM(K, W) BG_CUDA(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, Tile<W>::kSmemBytes))
+        BG_SMEM(gemm_bf16_kernel<kTN>, BLOCK_N); BG_SMEM(gemm_bf16_kernel<kNN>, BLOCK_N); BG_SMEM(gemm_bf16_kernel<kNT>, BLOCK_N);
+        BG_SMEM((gemm_bf16_kernel<kTN, kPlain, WIDE_N>), WIDE_N); BG_SMEM((gemm_bf16_kernel<kNN, kPlain, WIDE_N>), WIDE_N);
+        BG_SMEM((gemm_bf16_kernel<kNT, kPlain, WIDE_N>), WIDE_N);
+        BG_SMEM((gemm_bf16_kernel<kTN, kScatterMode>), BLOCK_N); BG_SMEM((gemm_bf16_kernel<kNN, kScatterMode>), BLOCK_N);
+        BG_SMEM((gemm_bf16_kernel<kNT, kScatterMode>), BLOCK_N);
+        BG_SMEM((gemm_bf16_kernel<kTN, kGatherMode>), BLOCK_N); BG_SMEM((gemm_bf16_kernel<kNN, kGatherMode>), BLOCK_N);
 #undef BG_SMEM
         g_num_sms = sms;
     }
@@ -464,12 +558,13 @@ static int gemm_setup() {
 
 
 
-static int make_ab_maps(CUtensorMap* ma, CUtensorMap* mb, const void* a, const void* b, long long m, long long n, long long k, int layout) {
+static int make_ab_maps(CUtensorMap* ma, CUtensorMap* mb, const void* a, const void* b, long long m, long long n, long long k, int layout,
+                        int block_n = BLOCK_N) {
     // A: TN/NN stored [M][K] (K-major: box 64 K x 128 rows); NT stored [K][M] (MN-major: box 64 M x 64 K-rows)
     int rc = layout == kNT ? make_map(ma, a, k, m, 64, BLOCK_K) : make_map(ma, a, m, k, BLOCK_K, BLOCK_M);
     if (rc) return rc;
-    // B: TN stored [N][K] (box 64 K x BLOCK_N rows); NN/NT stored [K][N] (box 64 N x 64 K-rows)
-    return layout == kTN ? make_map(mb, b, n, k, BLOCK_K, BLOCK_N) : make_map(mb, b, k, n, 64, BLOCK_K);
+    // B: TN stored [N][K] (box 64 K x block_n rows); NN/NT stored [K][N] (box 64 N x 64 K-rows)
+    return layout == kTN ? make_map(mb, b, n, k, BLOCK_K, block_n) : make_map(mb, b, k, n, 64, BLOCK_K);
 }
 
 static int gemm_launch(const void* a, const void* b, void* c, const void* addend, long long m, long long n, long long k, int layout, void* stream);
@@ -487,31 +582,43 @@ extern "C" int bg_gemm_bf16_add(const void* a, const void* b, void* c, const voi
     return gemm_launch(a, b, c, addend, m, n, k, layout, stream);
 }
 
+template <int kBlockN>
+static int plain_launch(const void* a, const void* b, void* c, const void* addend, long long m, long long n, long long k, int layout, void* stream);
+
 static int gemm_launch(const void* a, const void* b, void* c, const void* addend, long long m, long long n, long long k, int layout, void* stream) {
-    const int accumulate = addend != nullptr;
     if (layout < 0 || layout > 2) return fail(BG_EINVAL, "bg_gemm_bf16: layout %d", layout);
     if (m <= 0 || n <= 0 || k <= 0 || m % 8 || n % 8 || k % 8)
         return fail(BG_EINVAL, "bg_gemm_bf16: m,n,k (%lld,%lld,%lld) must be positive multiples of 8", m, n, k);
     if (((uintptr_t)a | (uintptr_t)b | (uintptr_t)c) % 16) return fail(BG_EINVAL, "bg_gemm_bf16: pointers must be 16-B aligned");
+    // 256-wide tiles for every output wider than one 128-wide tile; at N <= 128 a 256-wide tile would compute half zeros
+    return n > BLOCK_N ? plain_launch<WIDE_N>(a, b, c, addend, m, n, k, layout, stream)
+                       : plain_launch<BLOCK_N>(a, b, c, addend, m, n, k, layout, stream);
+}
+
+template <int kBlockN>
+static int plain_launch(const void* a, const void* b, void* c, const void* addend, long long m, long long n, long long k, int layout, void* stream) {
     CUtensorMap ma, mb, mc;
-    int rc = make_ab_maps(&ma, &mb, a, b, m, n, k, layout);
+    int rc = make_ab_maps(&ma, &mb, a, b, m, n, k, layout, kBlockN);
     if (rc) return rc;
     rc = make_map(&mc, c, m, n, kStoreCols, BLOCK_M);
     if (rc) return rc;
     rc = gemm_setup();
     if (rc) return rc;
-    const long long n_blocks = (n + BLOCK_N - 1) / BLOCK_N, tiles = ((m + BLOCK_M - 1) / BLOCK_M) * n_blocks;
+    const long long n_blocks = (n + kBlockN - 1) / kBlockN, tiles = ((m + BLOCK_M - 1) / BLOCK_M) * n_blocks;
     const int grid = (int)(tiles < g_num_sms ? tiles : g_num_sms);
     cudaStream_t st = (cudaStream_t)stream;
     const __nv_bfloat16* c_old = (const __nv_bfloat16*)addend;
-    // Raster: m-blocks per sweep over n.  From a sweep of 1..64 at the flagship shapes on H100 (DESIGN section 4): outputs of
-    // <= 32 n-blocks run fastest (or within 3 %) with 2, wider ones within 5 % of their best with 8; the fused modes' 16 took up to
-    // 1.58x as long.  The raster orders tiles only; every output element is the same.
+    const int accumulate = addend != nullptr;
+    constexpr int smem = Tile<kBlockN>::kSmemBytes;
+    // Raster: m-blocks per sweep over n.  From a sweep of 1..64 with the 256-wide tile at the flagship shapes on H100 (DESIGN
+    // section 4): outputs of <= 16 n-blocks (N <= 4096) run within 3.4 % of their best with 4, wider ones within 1.5 % with 16.
+    // At N <= 128 (one n-block, the 128-wide tile) every group size walks the same order.  The raster orders tiles only; every
+    // output element is the same.
     FuseParams<kPlain> plain;
-    plain.group_m = n_blocks <= 32 ? 2 : 8;
-    if (layout == kTN) gemm_bf16_kernel<kTN><<<grid, kThreads, kSmemBytes, st>>>(ma, mb, mc, c_old, (int)m, (int)n, (int)k, accumulate, plain);
-    else if (layout == kNN) gemm_bf16_kernel<kNN><<<grid, kThreads, kSmemBytes, st>>>(ma, mb, mc, c_old, (int)m, (int)n, (int)k, accumulate, plain);
-    else gemm_bf16_kernel<kNT><<<grid, kThreads, kSmemBytes, st>>>(ma, mb, mc, c_old, (int)m, (int)n, (int)k, accumulate, plain);
+    plain.group_m = n_blocks <= 16 ? 4 : 16;
+    if (layout == kTN) gemm_bf16_kernel<kTN, kPlain, kBlockN><<<grid, kThreads, smem, st>>>(ma, mb, mc, c_old, (int)m, (int)n, (int)k, accumulate, plain);
+    else if (layout == kNN) gemm_bf16_kernel<kNN, kPlain, kBlockN><<<grid, kThreads, smem, st>>>(ma, mb, mc, c_old, (int)m, (int)n, (int)k, accumulate, plain);
+    else gemm_bf16_kernel<kNT, kPlain, kBlockN><<<grid, kThreads, smem, st>>>(ma, mb, mc, c_old, (int)m, (int)n, (int)k, accumulate, plain);
     BG_CHECK_LAUNCH();
     return BG_OK;
 }
@@ -630,9 +737,9 @@ int bg_gemm_scatter_launch(const void* a, const void* b, long long m, long long 
     const int grid = (int)(tiles < g_num_sms ? tiles : g_num_sms);
     const int local_tiles = (rows_per_rank / BLOCK_M) * n_blocks;
     const CUtensorMap& mc_unused = sp.dst[0];
-    if (layout == kTN) gemm_bf16_kernel<kTN, kScatterMode><<<grid, kThreads, kSmemBytes, st>>>(ma, mb, mc_unused, nullptr, (int)m, (int)n, (int)k, 0, sp);
-    else if (layout == kNN) gemm_bf16_kernel<kNN, kScatterMode><<<grid, kThreads, kSmemBytes, st>>>(ma, mb, mc_unused, nullptr, (int)m, (int)n, (int)k, 0, sp);
-    else gemm_bf16_kernel<kNT, kScatterMode><<<grid, kThreads, kSmemBytes, st>>>(ma, mb, mc_unused, nullptr, (int)m, (int)n, (int)k, 0, sp);
+    if (layout == kTN) gemm_bf16_kernel<kTN, kScatterMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(ma, mb, mc_unused, nullptr, (int)m, (int)n, (int)k, 0, sp);
+    else if (layout == kNN) gemm_bf16_kernel<kNN, kScatterMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(ma, mb, mc_unused, nullptr, (int)m, (int)n, (int)k, 0, sp);
+    else gemm_bf16_kernel<kNT, kScatterMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(ma, mb, mc_unused, nullptr, (int)m, (int)n, (int)k, 0, sp);
     BG_CHECK_LAUNCH();
     // one reducer CTA fits beside a GEMM CTA (registers); more CTAs than SMs only queue
     const int rgrid = local_tiles < g_num_sms ? local_tiles : g_num_sms;
@@ -674,8 +781,8 @@ int bg_gemm_gather_launch(const void* a_local, const void* a_staged, const void*
     if (rc) return rc;
     const long long tiles = (m / BLOCK_M) * ((n + BLOCK_N - 1) / BLOCK_N);
     const int grid = (int)(tiles < g_num_sms ? tiles : g_num_sms);
-    if (layout == kTN) gemm_bf16_kernel<kTN, kGatherMode><<<grid, kThreads, kSmemBytes, st>>>(ma, mb, mc, nullptr, (int)m, (int)n, (int)k, 0, gp);
-    else gemm_bf16_kernel<kNN, kGatherMode><<<grid, kThreads, kSmemBytes, st>>>(ma, mb, mc, nullptr, (int)m, (int)n, (int)k, 0, gp);
+    if (layout == kTN) gemm_bf16_kernel<kTN, kGatherMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(ma, mb, mc, nullptr, (int)m, (int)n, (int)k, 0, gp);
+    else gemm_bf16_kernel<kNN, kGatherMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(ma, mb, mc, nullptr, (int)m, (int)n, (int)k, 0, gp);
     BG_CHECK_LAUNCH();
     return BG_OK;
 }

@@ -39,8 +39,8 @@ FLAGSHIP_GEMMS = [
 
 def gemm():
     """The flagship GEMMs, ours and cuBLAS (torch) interleaved round by round, on input sets rotated so that their sum exceeds
-    the 50 MB L2.  operand_TBps = the A and B bytes the CTAs load from L2 into shared memory (tiles x k-blocks x 32 KiB) over
-    the kernel time."""
+    the 50 MB L2.  operand_TBps = the A and B bytes the CTAs load from L2 into shared memory (tiles x k-blocks x (128 + tile
+    width) x 64 x 2 B: 32 KiB for a 128-wide tile, 48 KiB for a 256-wide one) over the kernel time."""
     import math
     import subprocess
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -98,8 +98,10 @@ def gemm():
             rec[name + "_ms"] = round(t, 4)
             rec[name + "_tflops"] = round(fl / t / 1e9, 1)
             rec[name + "_spread_pct"] = round(100 * (max(ts) - min(ts)) / t, 1)
-        tiles_kblocks = -(-m // 128) * -(-n // 128) * -(-k // 64)
-        rec["ours_operand_TBps"] = round(tiles_kblocks * 32768 / rec["ours_ms"] / 1e9, 2)
+        bn = 256 if n > 128 else 128    # the plain GEMM's tile width for this N (gemm_launch in bg_gemm.cu)
+        tiles_kblocks = -(-m // 128) * -(-n // bn) * -(-k // 64)
+        rec["ours_tile_n"] = bn
+        rec["ours_operand_TBps"] = round(tiles_kblocks * (128 + bn) * 64 * 2 / rec["ours_ms"] / 1e9, 2)
         print(json.dumps(rec), flush=True)
         del sets
         torch.cuda.empty_cache()
