@@ -221,12 +221,13 @@ def _reserve_activation_staging(be, args, info, hp_whole, hp_model, tp_groups, s
             if lst:
                 reserve(lst[i])
     # cp_comm="ring": receive slots of their own per cp group, for the largest local K block (microbatch x s/c x kv heads x head dim)
-    # of this stage's context-parallel layers -- 2 x (K + V) bf16 + 2 x (dK + dV) fp32, more than the staging estimate above
+    # of this stage's context-parallel layers -- 2 x (K + V) bf16 + 2 x (dK + dV) fp32, more than the staging estimate above.  On a
+    # layer that also runs Ulysses the block carries the K/V heads left after the exchange (kv_heads_attn: ng/p, or n/p replicated)
     ring_elems = {}
     for m in hp_model.modules():
         if isinstance(m, ParallelAttention) and m.use_cp and m.cp_comm == "ring" and m.cp_group is not None and m.cp_group.size > 1:
             key = tuple(m.cp_group.ranks)
-            elems = max_mbs * (seq // m.cp_group.size) * m.ng_local * m.hn
+            elems = max_mbs * (seq // m.cp_group.size) * m.kv_heads_attn * m.hn
             ring_elems[key] = (m.cp_group, max(elems, ring_elems.get(key, (None, 0))[1]))
     for group, elems in ring_elems.values():
         be.reserve_cp_ring(group, elems)

@@ -32,8 +32,32 @@ def _zigzag_transformation(x, cp):
     if cp == 1:
         return x
     assert 2 * cp <= x.shape[0], "sequence length must be larger than 2*cp"
+    # chunk views concatenated: an index tensor built on the host would be a copy that synchronises the stream with the host in
+    # every context-parallel layer (and, with virtual ranks on one device, would wait on a peer whose work is not issued yet)
     chunks = x.reshape(2 * cp, -1, *x.shape[1:])
-    return chunks[torch.tensor(_zigzag_indices(cp), device=x.device)].reshape(-1, *x.shape[1:])
+    return torch.cat([chunks[i] for i in _zigzag_indices(cp)]).reshape(-1, *x.shape[1:])
+
+
+def local_positions(seq, cp=1, cp_rank=0, sp=1, sp_rank=0):
+    """Global token positions of the rows one rank holds of a ``seq``-token sequence, in row order (LongTensor).
+
+    The reference's layout for zigzag context parallelism composed with Ulysses (``get_pos_emb_on_this_cp_sp_rank_galvatron``,
+    megatron/core/models/common/embeddings/rotary_pos_embedding.py:33-56): cp rank r holds chunks (r, 2cp-1-r) of 2cp equal chunks,
+    and sp rank j holds the j-th of ``sp`` contiguous slices of those two chunks concatenated (a slice straddles the two chunks when
+    ``sp`` is odd).  Tokens, labels, RoPE tables and relocation all follow it: the relocation gathers over tp_sp_cp groups whose
+    rank order is sp-minor, which is this order."""
+    if cp == 1:
+        if seq % sp:
+            raise ValueError("sequence length %d is not a multiple of the sequence-parallel degree %d" % (seq, sp))
+        idx = torch.arange(seq)
+    else:
+        half = seq // (2 * cp)
+        if seq % (2 * cp * sp):
+            raise ValueError("sequence length %d is not a multiple of 2 x cp x sp = %d" % (seq, 2 * cp * sp))
+        idx = torch.cat([torch.arange(cp_rank * half, (cp_rank + 1) * half),
+                         torch.arange((2 * cp - 1 - cp_rank) * half, (2 * cp - cp_rank) * half)])
+    n = idx.numel() // sp
+    return idx[sp_rank * n:(sp_rank + 1) * n]
 
 
 def _reverse_zigzag_transformation(x, cp):
@@ -44,7 +68,7 @@ def _reverse_zigzag_transformation(x, cp):
     for pos, src in enumerate(fwd):
         inv[src] = pos
     chunks = x.reshape(2 * cp, -1, *x.shape[1:])
-    return chunks[torch.tensor(inv, device=x.device)].reshape(-1, *x.shape[1:])
+    return torch.cat([chunks[i] for i in inv]).reshape(-1, *x.shape[1:])
 
 
 def _gather_first_dim(x, group):

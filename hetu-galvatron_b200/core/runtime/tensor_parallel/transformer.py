@@ -358,6 +358,50 @@ class _CpRingAttnFn(torch.autograd.Function):
         return dq, dk, dv, None, None
 
 
+def cp_attention(q, k, v, group, scale, comm):
+    """Causal attention of a cp rank's zigzag rows [b, s/c, n, d] over the whole sequence, by the exchange ``comm`` names
+    (``cp_comm``: "allgather" or "ring")."""
+    if comm == "ring" and _size(group) > 1:
+        return _CpRingAttnFn.apply(q, k, v, group, scale)
+    return _cp_attention(q, k, v, group, scale)
+
+
+def _ulysses_to_heads(q, k, v, sp_group):
+    """[b, s/p, n, d] -> [b, s, n/p, d] in one exchange; K/V with fewer heads than p are first expanded to the query heads, as the
+    reference does (transformer.py:842-848)"""
+    p = sp_group.size
+    if k.shape[2] % p:
+        rep = q.shape[2] // k.shape[2]
+        k, v = k.repeat_interleave(rep, dim=2), v.repeat_interleave(rep, dim=2)
+    return _UlyssesFn.apply(sp_group, True, q, k, v)
+
+
+def ulysses_cp_attention(q, k, v, sp_group, cp_group, scale, comm):
+    """Ulysses and zigzag context parallelism on one layer (the reference wraps its zigzag ring in DistributedAttention,
+    transformer.py:641-654): this rank's rows [b, s/(c*p), n, d] -> the to-heads exchange over the sp group gives the cp rank's s/c
+    zigzag rows of n/p heads (the sp ranks hold contiguous slices of them, redistribute.local_positions), the cp exchange
+    attends them over the whole sequence, the inverse exchange returns [b, s/(c*p), n, d].  Only the existing kernels run."""
+    q, k, v = _ulysses_to_heads(q, k, v, sp_group)                      # [b, s/c, n/p, d]
+    ctxt = cp_attention(q, k, v, cp_group, scale, comm)
+    return _UlyssesFn.apply(sp_group, False, ctxt)[0]
+
+
+def _check_ulysses_cp(p, c, kv_row_bytes):
+    """Construction-time limits of a layer with both Ulysses (degree p) and context parallelism (degree c), beyond Ulysses' own
+    n_heads % p: the sequence splits into 2c zigzag chunks whose concatenated pairs split p ways, and every K/V row the exchanges
+    move is whole 16-byte vectors."""
+    try:
+        from ..arguments import get_args
+        seq = getattr(get_args(), "seq_length", None)
+    except RuntimeError:
+        seq = None
+    if seq is not None and seq % (2 * c * p):
+        raise ValueError("sequence length %d must be a multiple of 2 x cp x sp = %d when context parallelism (cp %d) and Ulysses "
+                         "(sp %d) share a layer" % (seq, 2 * c * p, c, p))
+    if kv_row_bytes % 16:
+        raise ValueError("a K/V row of %d bytes per token after the Ulysses exchange is not a multiple of 16 bytes" % kv_row_bytes)
+
+
 def _recompute_activations():
     try:
         from ..arguments import get_args
@@ -416,7 +460,8 @@ class ParallelMLP(nn.Module):
 
 
 class ParallelAttention(nn.Module):
-    """Self-attention with TP heads or Ulysses sequence parallelism (transformer.py:512-900)."""
+    """Self-attention with TP heads or Ulysses sequence parallelism, and zigzag context parallelism on its own or inside the Ulysses
+    exchange (transformer.py:512-900, :641-654)."""
 
     def __init__(self, config, layer_number, attention_type=AttnType.self_attn, attn_mask_type=AttnMaskType.padding,
                  tp_group=None, sp_group=None, cp_group=None, cp_ranks=None, use_ulysses=False, use_zigzag_cp=False,
@@ -426,8 +471,6 @@ class ParallelAttention(nn.Module):
             raise NotImplementedError("only self attention is on the Galvatron hot path")
         self.use_cp = bool(use_zigzag_cp) or _size(cp_group) > 1
         self.cp_comm = cp_comm_mode()
-        if self.use_cp and use_ulysses and _size(sp_group) > 1:
-            raise NotImplementedError("context parallelism together with Ulysses on the same layer is not supported")
         self.layer_number = max(1, layer_number)
         self.attn_mask_type = attn_mask_type
         self.tp_group, self.sp_group, self.cp_group = tp_group, sp_group, cp_group
@@ -442,6 +485,13 @@ class ParallelAttention(nn.Module):
             assert n_heads % sp_group.size == 0, "num_attention_heads must be divisible by the Ulysses degree"  # :642
         self.np_local, self.ng_local = n_heads // world, n_groups // world
         self.r = self.np_local // self.ng_local
+        # K/V heads of one rank at the attention call: after the Ulysses exchange ng/p, or n/p when K/V are replicated first
+        self.kv_heads_attn = self.ng_local
+        if self.use_ulysses:
+            p = sp_group.size
+            self.kv_heads_attn = (self.ng_local if self.ng_local % p == 0 else self.np_local) // p
+        if self.use_ulysses and self.use_cp:
+            _check_ulysses_cp(sp_group.size, _size(cp_group), self.kv_heads_attn * self.hn * 2)
         add_bias = bool(getattr(config, "add_bias_linear", False))       # GPT / BERT: biases on both projections (:600-640)
         self.query_key_value = ColumnParallelLinear(config.hidden_size, (n_heads + 2 * n_groups) * self.hn, config=config,
                                                     bias=add_bias, gather_output=False, tp_group=tp_group,
@@ -491,20 +541,16 @@ class ParallelAttention(nn.Module):
         # padding mask (BERT): [b, s] bool over the keys, True = attend (the reference builds the extended [b,1,1,s] additive
         # mask in bert_hf/BertModel_sequential.py and hands it to every layer)
         key_mask = attention_mask if (not causal and attention_mask is not None) else None
-        if self.use_ulysses:
-            p = self.sp_group.size
-            if self.ng_local % p:  # too few KV heads to scatter: expand as the reference does (:842-848)
-                rep = self.np_local // self.ng_local
-                k, v = k.repeat_interleave(rep, dim=2), v.repeat_interleave(rep, dim=2)
-            q, k, v = _UlyssesFn.apply(self.sp_group, True, q, k, v)       # [b, s, n/p, hn]
+        if self.use_cp:
+            assert causal, "context parallelism is implemented for causal self-attention"
+        if self.use_ulysses and self.use_cp:
+            ctxt = ulysses_cp_attention(q, k, v, self.sp_group, self.cp_group, self.softmax_scale, self.cp_comm)   # [b, s/(c*p), n, hn]
+        elif self.use_ulysses:
+            q, k, v = _ulysses_to_heads(q, k, v, self.sp_group)              # [b, s, n/p, hn]
             ctxt = self._core_attention(q, k, v, causal, key_mask)
             (ctxt,) = _UlyssesFn.apply(self.sp_group, False, ctxt)         # [b, s/p, n, hn]
         elif self.use_cp:
-            assert causal, "context parallelism is implemented for causal self-attention"
-            if self.cp_comm == "ring" and _size(self.cp_group) > 1:
-                ctxt = _CpRingAttnFn.apply(q, k, v, self.cp_group, self.softmax_scale)   # [b, s/c, np, hn]
-            else:
-                ctxt = _cp_attention(q, k, v, self.cp_group, self.softmax_scale)      # [b, s/c, np, hn]
+            ctxt = cp_attention(q, k, v, self.cp_group, self.softmax_scale, self.cp_comm)   # [b, s/c, np, hn]
         else:
             ctxt = self._core_attention(q, k, v, causal, key_mask)          # [b, s, np, hn]
         b, s = ctxt.shape[0], ctxt.shape[1]

@@ -5,7 +5,8 @@ import torch.nn as nn
 from ..core.runtime.arguments import get_args
 from ..core.runtime.hybrid_parallel_config import ModelInfo, mixed_precision_dtype
 from ..core.runtime.pipeline import PipeSequential
-from ..core.runtime.tensor_parallel import (RMSNorm, VocabUtility, copy_to_tensor_model_parallel_region_group,
+from ..core.runtime.redistribute import local_positions
+from ..core.runtime.tensor_parallel import (RMSNorm, copy_to_tensor_model_parallel_region_group,
                                             gather_from_tensor_model_parallel_region_group,
                                             linear_with_grad_accumulation_and_async_allreduce,
                                             scatter_to_sequence_parallel_region_group, vocab_parallel_cross_entropy)
@@ -15,16 +16,19 @@ def _size(g):
     return 1 if g is None else g.size
 
 
-def _zigzag_local(x, group):
-    """[b, s] tokens / labels -> this context-parallel rank's two zigzag chunks (r, 2c-1-r) [b, s/c].  The reference's real-data
-    loader does this slicing before the model (Megatron ``get_batch_on_this_cp_rank``, models/llama_hf/dataloader.py:151);
-    here the first and the last layer do it, so ``forward_backward`` takes the same full-sequence batch in every mode."""
-    c = _size(group)
-    if c == 1:
+def _zigzag_local(x, group, sp_group=None):
+    """[b, s] tokens / labels -> the tokens this rank holds [b, s/(c*p)]: the context-parallel rank's two zigzag chunks
+    (r, 2c-1-r), and of those the Ulysses rank's contiguous slice (redistribute.local_positions).  The reference's real-data
+    loader does this slicing before the model (Megatron ``get_batch_on_this_cp_rank``, models/llama_hf/dataloader.py:151,
+    then the vocab_sp slice :45-57); here the first and the last layer do it, so ``forward_backward`` takes the same
+    full-sequence batch in every mode."""
+    c, p = _size(group), _size(sp_group)
+    if c == 1 and p == 1:
         return x
-    r, half = group.rank_in_group(), x.shape[1] // (2 * c)
-    assert half * 2 * c == x.shape[1], "sequence length must be a multiple of 2 x the context-parallel degree"
-    return torch.cat([x[:, r * half:(r + 1) * half], x[:, (2 * c - 1 - r) * half:(2 * c - r) * half]], 1).contiguous()
+    idx = local_positions(x.shape[1], c, group.rank_in_group() if c > 1 else 0, p, sp_group.rank_in_group() if p > 1 else 0)
+    if c == 1:      # one contiguous slice
+        return x[:, int(idx[0]):int(idx[-1]) + 1].contiguous()
+    return x[:, idx.to(x.device)].contiguous()
 
 
 class LlamaEmbeddings_(nn.Module):
@@ -35,16 +39,11 @@ class LlamaEmbeddings_(nn.Module):
         self.sequence_parallel = args.sequence_parallel
         self.tp_group, self.sp_group, self.cp_group = (self.embed_tokens.tp_group, self.embed_tokens.sp_group,
                                                        self.embed_tokens.cp_group)
-        self.vocab_sp = args.vocab_sp
-        if self.vocab_sp:  # Ulysses on the embedding: each rank embeds its own sequence slice (:45-57)
-            seq = int(args.seq_length / _size(self.cp_group))
-            self.seq_start_index, self.seq_end_index = VocabUtility.vocab_range_from_global_vocab_size(
-                seq, self.sp_group.rank_in_group() if _size(self.sp_group) > 1 else 0, _size(self.sp_group))
+        # Ulysses on the embedding: each rank embeds its own sequence slice (:45-57)
+        self.seq_group = self.sp_group if args.vocab_sp else None
 
     def forward(self, tokens, position_ids=None, attention_mask=None, labels=None):
-        tokens = _zigzag_local(tokens, self.cp_group)
-        if self.vocab_sp:
-            tokens = tokens[:, self.seq_start_index:self.seq_end_index].contiguous()
+        tokens = _zigzag_local(tokens, self.cp_group, self.seq_group)
         hidden_states = self.embed_tokens(tokens)
         hidden_states = hidden_states.transpose(0, 1).contiguous()           # [b, s, h] -> [s, b, h]
         if self.sequence_parallel:
@@ -102,15 +101,10 @@ class LlamaCls_(nn.Module):
         self.parallel_loss = parallel_loss
         self.half_entropy = half_entropy and not args.entropy_in_fp32
         self.vocab_sp = args.vocab_sp
-        if self.vocab_sp:
-            seq = int(args.seq_length / _size(self.cp_group))
-            self.seq_start_index, self.seq_end_index = VocabUtility.vocab_range_from_global_vocab_size(
-                seq, self.sp_group.rank_in_group() if _size(self.sp_group) > 1 else 0, _size(self.sp_group))
+        self.seq_group = self.sp_group if self.vocab_sp else None
 
     def forward(self, hidden_states, position_ids=None, attention_mask=None, labels=None):
-        labels = _zigzag_local(labels, self.cp_group)
-        if self.vocab_sp:
-            labels = labels[:, self.seq_start_index:self.seq_end_index].contiguous()
+        labels = _zigzag_local(labels, self.cp_group, self.seq_group)
         # (without SP the dgrad all-reduce of copy_to_tensor_model_parallel_region :146-147 happens inside the linear)
         logits_parallel = self.lm_head(hidden_states)                          # [s, b, V/t]
         labels = labels.transpose(0, 1).contiguous()                            # [b, s] -> [s, b]

@@ -6,6 +6,7 @@ from torch import nn
 
 from ..core.runtime.arguments import get_args
 from ..core.runtime.backend import get_backend
+from ..core.runtime.redistribute import local_positions
 from ..core.runtime.tensor_parallel import (AttnMaskType, AttnType, ColumnParallelLinear, ParallelAttention, ParallelMLP,
                                             RMSNorm, VocabParallelEmbedding)
 
@@ -53,12 +54,14 @@ class LlamaAttention_tp(nn.Module):
         return self._rope_cache[key]
 
     def _rope_zigzag(self, local_seq, device):
+        """RoPE rows of the ``local_seq`` tokens this rank holds under zigzag context parallelism, Ulysses or not: the positions
+        of redistribute.local_positions (the reference builds them in get_pos_emb_on_this_cp_sp_rank_galvatron)"""
         key = ("zigzag", local_seq)
         if key not in self._rope_cache:
             c, r = self.cp_size, self.cp_group.rank_in_group()
-            cos, sin = self._rope(local_seq * c, 0, device)
-            half = local_seq // 2
-            idx = torch.cat([torch.arange(r * half, (r + 1) * half), torch.arange((2 * c - 1 - r) * half, (2 * c - r) * half)]).to(device)
+            p, j = (self.sp_size, self.sp_group.rank_in_group()) if self.use_ulysses else (1, 0)
+            cos, sin = self._rope(local_seq * c * p, 0, device)
+            idx = local_positions(local_seq * c * p, c, r, p, j).to(device)
             self._rope_cache[key] = (cos[idx].contiguous(), sin[idx].contiguous())
         return self._rope_cache[key]
 
@@ -75,8 +78,9 @@ class LlamaAttention_tp(nn.Module):
         else:
             seq, offset = s_local, 0
         if self.use_zigzag_cp:
-            # zigzag context parallelism: this rank's `seq` tokens are chunks (r, 2c-1-r) of the c*seq-token sequence; RoPE takes
-            # their global positions (the reference lets Megatron's RotaryEmbedding pick them, LlamaModel_tensor_parallel.py:59-63)
+            # zigzag context parallelism: this rank's `seq` tokens are chunks (r, 2c-1-r) of the sequence, or under Ulysses the sp
+            # rank's slice of them; RoPE takes their global positions (the reference lets Megatron's RotaryEmbedding pick them,
+            # LlamaModel_tensor_parallel.py:58-63)
             rope = self._rope_zigzag(seq, hidden_states.device)
         else:
             rope = self._rope(seq, offset, hidden_states.device)
