@@ -59,7 +59,6 @@ SIGNATURES = {
     "bg_group_mc_join": (_i, [_vp, _i, _i, _sz]),
     "bg_group_mc_bind": (_i, [_vp, _i, _sz]),
     "bg_group_mc_disable": (_i, [_vp, _i]),
-    "bg_all_reduce_nvls": (_i, [_vp, _i, _i, _sz, _vp, _sz, _i, _c.c_float, _vp]),
     "bg_group_create": (_i, [_vp, _c.POINTER(_i), _i, _c.POINTER(_i)]),
     "bg_group_info": (_i, [_vp, _i, _c.POINTER(_i), _c.POINTER(_i), _c.POINTER(_i)]),
     "bg_build_groups": (_i, [_i, _i, _i, _i, _c.POINTER(_i), _c.POINTER(_i), _c.POINTER(_i), _c.POINTER(_i),
@@ -408,20 +407,6 @@ class BgComm:
             check(lib().bg_group_create(self._ctx, arr, len(ranks), ctypes.byref(out)))
             gid = self._gids[tuple(ranks)] = out.value
         return gid
-
-    def has_nvls(self, group, buf=None, byte_offset=0, nbytes=0):
-        """Is ``group`` (and, if given, this range of its symmetric buffer) inside a multicast-bound arena range?"""
-        reg = self._nvls.get(tuple(group.ranks))
-        if reg is None or buf is None:
-            return reg is not None
-        return (buf.offsets is not None and len(set(int(o) for o in buf.offsets)) == 1 and buf.offset + byte_offset >= reg[0]
-                and buf.offset + byte_offset + nbytes <= reg[0] + reg[1])
-
-    def all_reduce_nvls(self, group, byte_offset, dst, elems, dtype, scale=1.0, lane=LANE_ACT, stream=None):
-        """In-switch all-reduce of ``elems`` values at ``byte_offset`` of the group's NVLS buffer -> ``dst`` (or in place)."""
-        with self._in_order(stream) as sp:
-            check(lib().bg_all_reduce_nvls(self._ctx, self.group_id(group), lane, int(byte_offset), _ptr(dst) if dst is not None else None,
-                                           int(elems), dtype_code(dtype), float(scale), sp))
 
     def close(self):
         if self._fd_channel is not None:

@@ -8,6 +8,7 @@ Host-logic tests run the same layer/schedule code on CPU by *injecting* a backen
 backend (``oracle/gloo_backend.py``) lives with the oracle, is never imported from here, and is only ever installed
 by tests/ and bench.py's reference arm.
 """
+import contextlib
 import os
 
 import torch
@@ -37,12 +38,90 @@ def reset_backend():
     _BACKEND = None
 
 
+class StagingLayout:
+    """Byte layout of a group's activation staging buffer reserved for ``n`` data bytes (a multiple of 256):
+
+      [0, n)                   region 0: general staging, the all-gather landing, the unfused GEMM output and the stage of
+                               ``all_gather_gemm``.  The unfused dgrad GEMM + collective writes here over the re-gathered input of
+                               the same layer, so that layer's wgrad GEMM must have read the input before.
+      [n, 2n)                  partial tiles of the fused GEMM + reduce-scatter / all-reduce
+      [2n, 3n)                 the fused all-reduce result, which every member's tile reducer broadcasts into
+      [3n, 3n + F/2)           per-tile arrival counters of the scattering GEMMs
+      [3n + F/2, 3n + F)       per-block arrival counters of the gathering GEMM
+
+    F = FLAG_BYTES; the buffer is 3n + F bytes.  The counters are zero at rest."""
+
+    FLAG_BYTES = 1 << 16
+    COUNTER_BYTES = FLAG_BYTES // 2        # each of the two counter blocks
+
+    def __init__(self, n):
+        self.n = n
+        self.partials = n
+        self.result = 2 * n
+        self.scatter_counters = 3 * n
+        self.gather_counters = 3 * n + self.COUNTER_BYTES
+        self.total = 3 * n + self.FLAG_BYTES
+
+
+# fusion pays when the GEMM lasts at least as long as the transfer of its output; below that the GEMM outruns NVLink and the fused
+# kernel only adds its reducer tail (thresholds from measurements on an earlier GPU; not re-measured on H100)
+FUSE_MIN_K = 3072          # GEMM + reduce-scatter
+FUSE_AR_MIN_K = 2048       # GEMM + all-reduce
+FUSE_ENV = {"gemm_rs": "HGB_FUSE_GEMM_RS", "gemm_ar": "HGB_FUSE_GEMM_AR", "ag_gemm": "HGB_FUSE_AG_GEMM"}
+
+
+def fusion_allowed(kind, m, n, k, p, data_bytes, on, force=False):
+    """Does the fused GEMM + collective ``kind`` ("gemm_rs", "gemm_ar" or "ag_gemm") run for the [m, n] = [m, k] x [k, n] GEMM
+    (m: the full, gathered / unscattered rows) on a group of ``p`` ranks whose staging buffer holds ``data_bytes`` (None: none
+    reserved)?  ``on``: the kind's switch is not "0"; ``force``: it is "force", which lifts the K threshold (k None: no threshold).
+    The fused kernels need M in whole 128-row tiles per rank and their arrival counters inside the staging buffer's counter block."""
+    if not on or p < 2 or m % (p * 128) or data_bytes is None:
+        return False
+    if kind == "ag_gemm":
+        return k % 8 == 0 and data_bytes >= 2 * m * k and 4 * (m // 128) <= StagingLayout.COUNTER_BYTES
+    tiles = (m // p // 128) * ((n + 127) // 128)
+    if kind == "gemm_rs":
+        min_k, counter_bytes = FUSE_MIN_K, StagingLayout.COUNTER_BYTES
+    else:
+        # half the block (the C side's limit is the whole block); raising it would move shapes onto the fused path
+        min_k, counter_bytes = FUSE_AR_MIN_K, StagingLayout.COUNTER_BYTES // 2
+    return (n % 8 == 0 and (k is None or k >= min_k or force) and data_bytes >= 2 * m * n
+            and 4 * tiles <= counter_bytes)
+
+
+class _SymBuffers:
+    """The backend's own symmetric (peer-visible) buffers, one per (purpose, group).  Every member reserves them identically before
+    ``exchange()``.  A larger request before then allocates a new buffer and leaves the smaller one in the arena (every member does
+    the same, so the arena layouts stay identical); after ``exchange()`` it raises."""
+
+    def __init__(self, comm):
+        self.comm = comm
+        self._bufs = {}            # (purpose, group ranks) -> (SymBuffer, size)
+
+    def reserve(self, purpose, group, size, nbytes):
+        """The ``purpose`` buffer of ``group`` for ``size`` (in the purpose's own unit); when the current one is smaller, allocates
+        ``nbytes``.  -> (buffer, allocated by this call)"""
+        key = (purpose, tuple(group.ranks))
+        cur = self._bufs.get(key)
+        if cur is not None and cur[1] >= size:
+            return cur[0], False
+        if cur is not None and cur[0].offsets is not None:
+            from ... import _bg
+            raise _bg.BgError("%s buffer of group %s holds %d, need %d (reserve before exchange())" % (purpose, key[1], cur[1], size))
+        buf = self.comm.sym_alloc(group, nbytes)
+        self._bufs[key] = (buf, size)
+        return buf, True
+
+    def get(self, purpose, group):
+        """-> (buffer, size) as reserved, or (None, 0)"""
+        return self._bufs.get((purpose, tuple(group.ranks)), (None, 0))
+
+
 class CudaBackend:
     """H100 backend: symmetric-memory communicator + fused kernels."""
 
     name = "cuda-sm90a"
     is_cuda = True
-    FLAG_BYTES = 1 << 16
 
     def __init__(self, comm=None, arena_bytes=None, device=None):
         from ... import _bg
@@ -54,6 +133,8 @@ class CudaBackend:
         self.device_index = _world.get_local_rank() % torch.cuda.device_count() if device is None else device
         torch.cuda.set_device(self.device_index)
         self.device = torch.device("cuda", self.device_index)
+        self.nvls = False
+        self.nvls_regions = {}     # group ranks -> multicast-bound arena range, set by exchange()
         if comm is None:
             if arena_bytes is None:
                 arena_bytes = int(os.environ.get("HGB_ARENA_BYTES", 0))
@@ -99,13 +180,13 @@ class CudaBackend:
         self.reduce_stream = torch.cuda.Stream(device=self.device, priority=-1)
         self.p2p_stream = torch.cuda.Stream(device=self.device, priority=-1)
         self.comm_stream = torch.cuda.Stream(device=self.device, priority=-1)  # push kernels of the fused all-gather + GEMM; overlapped gathers
-        self.fuse_gemm_rs = os.environ.get("HGB_FUSE_GEMM_RS", "1") != "0"
-        self.fuse_gemm_ar = os.environ.get("HGB_FUSE_GEMM_AR", "1") != "0"
-        self.fuse_ag_gemm = os.environ.get("HGB_FUSE_AG_GEMM", "1") != "0"
+        self.fuse = {kind: os.environ.get(env, "1") != "0" for kind, env in FUSE_ENV.items()}
         self.n_fused = {"gemm_rs": 0, "gemm_ar": 0, "ag_gemm": 0}
         self.comm_profile = None   # bench.py: {kind: [(start_event, end_event, algorithmic_bus_bytes)]} while timing the collectives
         self.attn_impl = os.environ.get("HGB_ATTN", "cudnn")
-        self._staging = {}  # group ranks -> SymBuffer
+        self._bufs = _SymBuffers(comm)
+        self._cp_rings = {}        # group ranks -> _CpRing
+        self.world_group = None    # the whole job as one group, once its staging is reserved (clip_grad_norm's all-reduce)
         self._scratch = {}
         self.gemm_profile = None   # bench.py: list of (start_event, end_event, flops) while timing the dominant kernel
         # RMSNorm / LayerNorm backward: one fp32 weight-gradient partial row per CTA, 3 CTAs of 256 threads x <= 76 registers per SM
@@ -128,32 +209,22 @@ class CudaBackend:
     def sym_alloc(self, group, nbytes):
         return self.comm.sym_alloc(group, nbytes)
 
-    NVLS_MIN_BYTES = 1 << 20     # below this the one-shot / two-shot peer kernels win (latency)
-
     def exchange(self):
         self.comm.exchange()
-        if getattr(self, "nvls", False):
+        if self.nvls:
             self.nvls_regions = self.comm.setup_nvls()
 
     def reserve_staging(self, group, nbytes):
-        """Per-group activation staging buffer (peer-visible).  Must be called (identically on all members) before
-        ``exchange()``; later requests larger than the reservation raise."""
+        """Per-group activation staging buffer (peer-visible, laid out as ``StagingLayout`` for ``nbytes`` rounded up to 256).  Must
+        be called (identically on all members) before ``exchange()``; later requests larger than the reservation raise."""
         if group is None or group.size == 1:
             return None
-        key = tuple(group.ranks)
-        cur = self._staging.get(key)
-        nbytes = (int(nbytes) + 255) // 256 * 256
-        if cur is None or cur.data_bytes < nbytes:
-            if cur is not None and cur.offsets is not None:
-                raise self.bg.BgError("staging buffer for group %s is %d B, need %d B (reserve before exchange())" % (key, cur.data_bytes, nbytes))
-            # three regions of `nbytes`: [0] general staging / all-gather landing, [1] partial tiles of the fused GEMM +
-            # reduce-scatter / all-reduce, [2] the all-reduce result every member broadcasts into; tail: arrival counters
-            # (first half: per-tile counters of the scattering GEMMs, second half: per-block counters of the gathering GEMM)
-            buf = self.comm.sym_alloc(group, 3 * nbytes + self.FLAG_BYTES)
-            buf.data_bytes = nbytes
-            buf.u8[3 * nbytes:].zero_()
-            self._staging[key] = buf
-        return self._staging[key]
+        layout = StagingLayout((int(nbytes) + 255) // 256 * 256)
+        buf, new = self._bufs.reserve("staging", group, layout.n, layout.total)
+        if new:
+            buf.layout = layout
+            buf.u8[layout.scatter_counters:].zero_()
+        return buf
 
     def reserve_cp_ring(self, group, elems):
         """Receive slots of the context-parallel ring for ``group`` (``cp_comm="ring"``): a region of their own, sized for a local
@@ -161,32 +232,25 @@ class CudaBackend:
         ``exchange()``, identically on every member."""
         if group is None or group.size == 1:
             return
-        rings = self.__dict__.setdefault("_cp_ring_bufs", {})
-        key = tuple(group.ranks)
         elems = (int(elems) + 7) // 8 * 8
-        cur = rings.get(key)
-        if cur is None or cur[1] < elems:
-            if cur is not None and cur[0].offsets is not None:
-                raise self.bg.BgError("cp ring slots of group %s are already exchanged" % (key,))
-            rings[key] = (self.comm.sym_alloc(group, _CpRing.slot_bytes(elems)), elems)
+        self._bufs.reserve("cp_ring", group, elems, _CpRing.slot_bytes(elems))
 
     def cp_ring(self, group):
         """The ring transport of ``group`` (one per group: its flags' first-use state is shared by every layer on the group)."""
         key = tuple(group.ranks)
-        rings = self.__dict__.setdefault("_cp_rings", {})
-        if key not in rings:
-            buf = self.__dict__.get("_cp_ring_bufs", {}).get(key)
+        if key not in self._cp_rings:
+            buf, elems = self._bufs.get("cp_ring", group)
             if buf is None:
                 raise self.bg.BgError("no cp ring slots reserved for group %s (models built with cp_comm='ring' reserve them)" % (key,))
-            rings[key] = _CpRing(self.comm, group, buf[0], buf[1], comm_stream=self.comm_stream, counts=self.n_fused)
-        return rings[key]
+            self._cp_rings[key] = _CpRing(self.comm, group, buf, elems, comm_stream=self.comm_stream, counts=self.n_fused)
+        return self._cp_rings[key]
 
     def lse_merge(self, blk_out, blk_lse, acc_out, acc_lse, final_out=None, row_off=0, init=False):
         self.bg.lse_merge(blk_out.contiguous(), blk_lse.contiguous(), acc_out, acc_lse, final_out, row_off, init)
 
     def staging(self, group, nbytes, byte_offset=0):
-        buf = self._staging.get(tuple(group.ranks))
-        if buf is None or buf.data_bytes < nbytes + byte_offset:
+        buf, n = self._bufs.get("staging", group)
+        if buf is None or n < nbytes + byte_offset:
             raise self.bg.BgError("no staging buffer of %d B reserved for group %s" % (nbytes + byte_offset, group.ranks))
         return buf
 
@@ -200,7 +264,7 @@ class CudaBackend:
 
     def _is_staging(self, t, buf):
         base = buf.u8.data_ptr()
-        return base <= t.data_ptr() < base + buf.data_bytes
+        return base <= t.data_ptr() < base + buf.layout.n
 
     def _stage(self, x, group, byte_offset=0):
         """Make ``x`` peer-visible: no-op when it already lives in the group's staging buffer."""
@@ -236,19 +300,31 @@ class CudaBackend:
         """The optimizer (current stream) has rewritten the masters: the unshard stream must see that."""
         self.unshard_stream.wait_stream(torch.cuda.current_stream())
 
-    def unit_reduce(self, unit, accumulate):
-        """C2/C3 on the reduce stream, ordered after the unit's backward on the current stream."""
+    @contextlib.contextmanager
+    def _on_reduce_stream(self, unit, kind=None):
+        """Run the body on the reduce stream, ordered after the work already queued on the current stream (the unit's backward);
+        with ``kind``, time it as that reduce-scatter of the unit's gradient."""
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream())
         with torch.cuda.stream(self.reduce_stream):
             self.reduce_stream.wait_event(ev)
-            if unit.dp_type != "ddp":
+            if kind is None:
+                yield
+            else:
                 d, gsz = unit.group.size, (4 if unit.reduce_dtype == torch.float32 else 2)
-                with self._timed("sdp_reduce_scatter", (d - 1) / d * unit.padded * gsz, self.reduce_stream):
-                    self.comm.reduce_scatter_acc(unit.group, unit.G, unit.reduce_dtype, unit.master_grad,
-                                                 shard_elems=unit.shard_elems, prescale=1.0 / unit.prediv,
-                                                 postscale=1.0 / unit.postdiv, accumulate=accumulate, lane=self.bg.LANE_REDUCE)
-            elif unit.group.size == 1:
+                with self._timed(kind, (d - 1) / d * unit.padded * gsz, self.reduce_stream):
+                    yield
+
+    def unit_reduce(self, unit, accumulate):
+        """C2/C3 on the reduce stream, ordered after the unit's backward on the current stream."""
+        if unit.dp_type != "ddp":
+            with self._on_reduce_stream(unit, "sdp_reduce_scatter"):
+                self.comm.reduce_scatter_acc(unit.group, unit.G, unit.reduce_dtype, unit.master_grad,
+                                             shard_elems=unit.shard_elems, prescale=1.0 / unit.prediv,
+                                             postscale=1.0 / unit.postdiv, accumulate=accumulate, lane=self.bg.LANE_REDUCE)
+            return
+        with self._on_reduce_stream(unit):
+            if unit.group.size == 1:
                 self.cast(unit.g_flat, unit.master_grad, accumulate=accumulate)
             else:  # DDP layers: all-reduce of the full flat gradient (_runtime_utils.py:932-950), then cast/accumulate
                 key = (unit.reduce_dtype, unit.padded)
@@ -263,21 +339,16 @@ class CudaBackend:
         """C2 with the AdamW epilogue (reduce stream): gradients are consumed in registers, no fp32 gradient shard.  ``clip_coef``
         (fp32 device scalar): the step pass of deferred clipping, the reduced gradient multiplied by it."""
         lr, b1, b2, eps, wd, step = opt.hyper()
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream())
-        with torch.cuda.stream(self.reduce_stream):
-            self.reduce_stream.wait_event(ev)
-            d, gsz = unit.group.size, (4 if unit.reduce_dtype == torch.float32 else 2)
-            with self._timed("sdp_reduce_scatter_adamw", (d - 1) / d * unit.padded * gsz, self.reduce_stream):
-                if clip_coef is None:
-                    self.comm.reduce_scatter_adamw(unit.group, unit.G, unit.reduce_dtype, unit.flat_param.data, unit.exp_avg,
-                                                   unit.exp_avg_sq, unit.shard_elems, 1.0 / unit.prediv, 1.0 / unit.postdiv, lr, b1, b2,
-                                                   eps, wd, step, lane=self.bg.LANE_REDUCE)
-                else:
-                    self.comm.reduce_scatter_adamw_clipped(unit.group, unit.G, unit.reduce_dtype, unit.flat_param.data, unit.exp_avg,
-                                                           unit.exp_avg_sq, unit.shard_elems, 1.0 / unit.prediv, 1.0 / unit.postdiv, lr,
-                                                           b1, b2, eps, wd, step, clip_coef, lane=self.bg.LANE_REDUCE)
-                    self.n_fused["rs_adamw_clipped"] = self.n_fused.get("rs_adamw_clipped", 0) + 1
+        with self._on_reduce_stream(unit, "sdp_reduce_scatter_adamw"):
+            if clip_coef is None:
+                self.comm.reduce_scatter_adamw(unit.group, unit.G, unit.reduce_dtype, unit.flat_param.data, unit.exp_avg,
+                                               unit.exp_avg_sq, unit.shard_elems, 1.0 / unit.prediv, 1.0 / unit.postdiv, lr, b1, b2,
+                                               eps, wd, step, lane=self.bg.LANE_REDUCE)
+            else:
+                self.comm.reduce_scatter_adamw_clipped(unit.group, unit.G, unit.reduce_dtype, unit.flat_param.data, unit.exp_avg,
+                                                       unit.exp_avg_sq, unit.shard_elems, 1.0 / unit.prediv, 1.0 / unit.postdiv, lr,
+                                                       b1, b2, eps, wd, step, clip_coef, lane=self.bg.LANE_REDUCE)
+                self._count("rs_adamw_clipped")
 
     def clip_partials(self, n_units):
         """Zeroed fp32 [n_units, k]: one row per unit for the norm pass's per-warp sums of squares (4 warps x the largest grid)."""
@@ -288,22 +359,20 @@ class CudaBackend:
         """Norm pass of deferred clipping (reduce stream): the unit's reduce-scatter, whose epilogue only writes the per-warp sums of
         squares of the reduced gradient into ``partials`` (leaving out the shard-relative ranges ``skip``); ``into_master``: also
         the fp32 gradient shard (units whose G cannot be read again at the step)."""
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream())
-        with torch.cuda.stream(self.reduce_stream):
-            self.reduce_stream.wait_event(ev)
-            d, gsz = unit.group.size, (4 if unit.reduce_dtype == torch.float32 else 2)
-            with self._timed("sdp_reduce_scatter_sumsq", (d - 1) / d * unit.padded * gsz, self.reduce_stream):
-                self.comm.reduce_scatter_sumsq(unit.group, unit.G, unit.reduce_dtype, unit.shard_elems, 1.0 / unit.prediv,
-                                               1.0 / unit.postdiv, partials, skip, dst=unit.master_grad if into_master else None,
-                                               lane=self.bg.LANE_REDUCE)
-        self.n_fused["rs_sumsq"] = self.n_fused.get("rs_sumsq", 0) + 1
+        with self._on_reduce_stream(unit, "sdp_reduce_scatter_sumsq"):
+            self.comm.reduce_scatter_sumsq(unit.group, unit.G, unit.reduce_dtype, unit.shard_elems, 1.0 / unit.prediv,
+                                           1.0 / unit.postdiv, partials, skip, dst=unit.master_grad if into_master else None,
+                                           lane=self.bg.LANE_REDUCE)
+        self._count("rs_sumsq")
 
     def unit_adamw_clipped(self, unit, opt, clip_coef):
         """The clipped AdamW step on the unit's fp32 gradient shard (current stream, after ``finish_reductions``)."""
         lr, b1, b2, eps, wd, step = opt.hyper()
         self.bg.adamw_clipped(unit.flat_param.data, unit.exp_avg, unit.exp_avg_sq, unit.master_grad, lr, b1, b2, eps, wd, step, clip_coef)
-        self.n_fused["adamw_clipped"] = self.n_fused.get("adamw_clipped", 0) + 1
+        self._count("adamw_clipped")
+
+    def _count(self, kind):
+        self.n_fused[kind] = self.n_fused.get(kind, 0) + 1
 
     def finish_reductions(self):
         torch.cuda.current_stream().wait_stream(self.reduce_stream)
@@ -313,20 +382,15 @@ class CudaBackend:
         """Peer-visible landing buffer for ``gather_master`` (one per group, sized for its largest unit); before ``exchange()``."""
         if group is None or group.size == 1:
             return
-        bufs = self.__dict__.setdefault("_ckpt_bufs", {})
-        key = tuple(group.ranks)
-        cur = bufs.get(key)
-        if cur is None or cur.nbytes < nbytes:
-            if cur is not None and cur.offsets is not None:
-                raise self.bg.BgError("checkpoint gather buffer for group %s is already exchanged" % (key,))
-            bufs[key] = self.comm.sym_alloc(group, int(nbytes))
+        # its size is what sym_alloc allocates for the request (a whole number of 256-byte blocks)
+        self._bufs.reserve("checkpoint_gather", group, (int(nbytes) + 255) // 256 * 256, int(nbytes))
 
     def gather_master(self, unit):
         """Full fp32 flat parameter of ``unit`` on every member of its group (collective)."""
         if unit.dp_type == "ddp" or unit.group.size == 1:
             return unit.flat_param.data
-        buf = self.__dict__.get("_ckpt_bufs", {}).get(tuple(unit.group.ranks))
-        if buf is None or buf.nbytes < unit.padded * 4:
+        buf, nbytes = self._bufs.get("checkpoint_gather", unit.group)
+        if buf is None or nbytes < unit.padded * 4:
             raise self.bg.BgError("no checkpoint gather buffer reserved for group %s: construct the model with args.save set" % (unit.group.ranks,))
         self.comm.all_gather_cast(unit.group, unit.flat_param.data, buf, shard_elems=unit.shard_elems, lane=self.bg.LANE_MISC,
                                   dst_dtype=torch.float32)
@@ -373,21 +437,6 @@ class CudaBackend:
             self.comm.all_reduce(group, buf, out, elems=x.numel(), op=self.bg.MAX if op == "max" else self.bg.SUM,
                                  src_byte_offset=off)
         return out
-
-    def all_reduce_inplace(self, x, group):
-        """Sum ``x`` over ``group`` IN PLACE when that is possible without a copy: NVLS is on (and HGB_NVLS_INPLACE=1), ``x`` is a
-        contiguous view of the group's multicast-bound staging buffer and large enough.  Returns whether it did."""
-        if not (getattr(self, "nvls", False) and os.environ.get("HGB_NVLS_INPLACE", "0") == "1" and self.comm.has_nvls(group)):
-            return False
-        buf = self._staging.get(tuple(group.ranks))
-        nbytes = x.numel() * x.element_size()
-        if (buf is None or not x.is_contiguous() or not self._is_staging(x, buf) or x.dtype not in (torch.bfloat16, torch.float32)
-                or nbytes < self.NVLS_MIN_BYTES or nbytes % 16
-                or not self.comm.has_nvls(group, buf, x.data_ptr() - buf.u8.data_ptr(), nbytes)):
-            return False
-        region = self.comm._nvls[tuple(group.ranks)]
-        self.comm.all_reduce_nvls(group, x.data_ptr() - self.comm.arena_ptr - region[0], None, x.numel(), x.dtype)
-        return True
 
     def _all_reduce_padded(self, x, group, op, out):
         n = x.numel()
@@ -498,15 +547,20 @@ class CudaBackend:
         return outs
 
     # ---- math ops --------------------------------------------------------------------------------------------
-    def gemm(self, a, b, layout, out=None, accumulate=False, m=None, n=None, k=None, addend=None):
-        """bf16 GEMM on wgmma.  layout 'tn': a[M,K] b[N,K]; 'nn': a[M,K] b[K,N]; 'nt': a[K,M] b[K,N].
-        ``addend`` [M,N]: out = A op B + addend in the epilogue (the residual add behind a projection, one rounding)."""
+    @staticmethod
+    def _mnk(a, b, layout):
+        """-> (layout code, M, N, K) of A op B.  layout 'tn': a[M,K] b[N,K]; 'nn': a[M,K] b[K,N]; 'nt': a[K,M] b[K,N]."""
         code = {"tn": 0, "nn": 1, "nt": 2}[layout]
         if code == 2:
             k_, m_ = a.shape
         else:
             m_, k_ = a.shape
-        n_ = b.shape[0] if code == 0 else b.shape[1]
+        return code, m_, (b.shape[0] if code == 0 else b.shape[1]), k_
+
+    def gemm(self, a, b, layout, out=None, accumulate=False, addend=None):
+        """bf16 GEMM on wgmma (layouts: ``_mnk``).
+        ``addend`` [M,N]: out = A op B + addend in the epilogue (the residual add behind a projection, one rounding)."""
+        code, m_, n_, k_ = self._mnk(a, b, layout)
         if out is None:
             out = torch.empty(m_, n_, dtype=torch.bfloat16, device=a.device)
         if a.dtype != torch.bfloat16 or b.dtype != torch.bfloat16 or out.dtype != torch.bfloat16:
@@ -530,93 +584,65 @@ class CudaBackend:
             launch()
         return out
 
-    # fusion pays when the GEMM lasts at least as long as the transfer of its output; below that the GEMM outruns NVLink and the fused
-    # kernel only adds its reducer tail (thresholds from measurements on an earlier GPU; not re-measured on H100)
-    FUSE_MIN_K = 3072
-
-    def can_fuse_gemm_rs(self, m, n, group, k=None):
+    # ---- GEMM + collective: one fused operation where ``fusion_allowed`` says so, else the GEMM into the group's staging buffer
+    # followed by the stand-alone collective ------------------------------------------------------------------------------------------
+    def fuses(self, kind, m, n, k, group):
+        """Would the fused ``kind`` ("gemm_rs", "gemm_ar", "ag_gemm") run for the [m, n] = [m, k] x [k, n] GEMM over ``group``?
+        The on/off switches are read when the backend is built, "force" at every call."""
         p = 1 if group is None else group.size
-        if not self.fuse_gemm_rs or p < 2 or m % (p * 128) or n % 8:
-            return False
-        if k is not None and k < self.FUSE_MIN_K and os.environ.get("HGB_FUSE_GEMM_RS") != "force":
-            return False
-        buf = self._staging.get(tuple(group.ranks))
-        tiles = (m // p // 128) * ((n + 127) // 128)
-        return buf is not None and buf.data_bytes >= m * n * 2 and tiles * 4 <= self.FLAG_BYTES // 2
-
-    FUSE_AR_MIN_K = 2048   # as FUSE_MIN_K, for the fused GEMM + all-reduce
-
-    @staticmethod
-    def _mnk(a, b, layout):
-        code = {"tn": 0, "nn": 1, "nt": 2}[layout]
-        if code == 2:
-            k_, m_ = a.shape
-        else:
-            m_, k_ = a.shape
-        return code, m_, (b.shape[0] if code == 0 else b.shape[1]), k_
-
-    def can_fuse_gemm_ar(self, m, n, group, k=None):
-        p = 1 if group is None else group.size
-        if not self.fuse_gemm_ar or p < 2 or m % (p * 128) or n % 8:
-            return False
-        if k is not None and k < self.FUSE_AR_MIN_K and os.environ.get("HGB_FUSE_GEMM_AR") != "force":
-            return False
-        buf = self._staging.get(tuple(group.ranks))
-        tiles = (m // p // 128) * ((n + 127) // 128)
-        return buf is not None and buf.data_bytes >= m * n * 2 and tiles * 4 <= self.FLAG_BYTES // 2 // 2
-
-    def gemm_all_reduce(self, a, b, layout, group):
-        """[M, N] = sum over ``group`` of A op B, on every member (GEMM + C5/C6 in one operation): partial tiles go to their
-        owner's HBM, the owner's tile reducer sums them as they land and broadcasts the rows into every member's result."""
-        code, m_, n_, k_ = self._mnk(a, b, layout)
-        buf = self.staging(group, m_ * n_ * 2)
-        r = buf.data_bytes
-        with self._timed("gemm_all_reduce", 2.0 * (group.size - 1) / group.size * m_ * n_ * 2, flops=2.0 * m_ * n_ * k_):
-            self.comm.gemm_all_reduce(group, a, b, m_, n_, k_, code, buf, r, 3 * r, 2 * r)
-        self.n_fused["gemm_ar"] += 1
-        # the symmetric result buffer is rewritten by the next fused all-reduce of this group: hand out a private copy
-        return buf.u8[2 * r: 2 * r + m_ * n_ * 2].view(torch.bfloat16).view(m_, n_).clone()
-
-    def can_fuse_ag_gemm(self, m, k, group):
-        p = 1 if group is None else group.size
-        if not self.fuse_ag_gemm or p < 2 or m % (p * 128) or k % 8:
-            return False
-        buf = self._staging.get(tuple(group.ranks))
-        return buf is not None and buf.data_bytes >= m * k * 2 and (m // 128) * 4 <= self.FLAG_BYTES // 2
-
-    def all_gather_gemm(self, a_local, b, layout, group):
-        """out[M, N] = gather_rows(a_local[M/p, K]) op B (C7 + GEMM in one operation).  Returns (out, gathered A) -- the gathered
-        operand sits complete in the group's staging buffer afterwards (the wgrad GEMM of the same layer reads it there)."""
-        p = group.size
-        code = {"tn": 0, "nn": 1}[layout]
-        ml, k_ = a_local.shape
-        m_ = ml * p
-        n_ = b.shape[0] if code == 0 else b.shape[1]
-        buf = self.staging(group, m_ * k_ * 2)
-        out = torch.empty(m_, n_, dtype=torch.bfloat16, device=a_local.device)
-        with self._timed("all_gather_gemm", (p - 1) / p * m_ * k_ * 2, flops=2.0 * m_ * n_ * k_):
-            self.comm.all_gather_gemm(group, a_local, b, out, m_, n_, k_, code, buf, 0, 3 * buf.data_bytes + self.FLAG_BYTES // 2,
-                                      self.comm_stream)
-        a_local.record_stream(self.comm_stream)
-        self.n_fused["ag_gemm"] += 1
-        return out, buf.u8[: m_ * k_ * 2].view(torch.bfloat16).view(m_, k_)
+        buf, data_bytes = self._bufs.get("staging", group) if p > 1 else (None, 0)
+        return fusion_allowed(kind, m, n, k, p, None if buf is None else data_bytes, self.fuse[kind],
+                              os.environ.get(FUSE_ENV[kind]) == "force")
 
     def gemm_reduce_scatter(self, a, b, layout, group):
-        """[M, N] = A op B, reduce-scattered along M over ``group`` -> [M/p, N]: the wgmma GEMM's epilogue stores each
+        """[M, N] = A op B, reduce-scattered along M over ``group`` -> [M/p, N].  Fused: the wgmma GEMM's epilogue stores each
         partial tile into the owning rank's HBM and a tile reducer sums them as they land (GEMM + C8 in one operation)."""
-        code = {"tn": 0, "nn": 1, "nt": 2}[layout]
-        if code == 2:
-            k_, m_ = a.shape
-        else:
-            m_, k_ = a.shape
-        n_ = b.shape[0] if code == 0 else b.shape[1]
+        code, m_, n_, k_ = self._mnk(a, b, layout)
+        if not self.fuses("gemm_rs", m_, n_, k_, group):
+            staged, _ = self.staging_tensor(group, (m_, n_), a.dtype)
+            self.gemm(a, b, layout, out=staged)
+            return self.reduce_scatter_first_dim(staged, group)
         buf = self.staging(group, m_ * n_ * 2)
         out = torch.empty(m_ // group.size, n_, dtype=torch.bfloat16, device=a.device)
         with self._timed("gemm_reduce_scatter", (group.size - 1) / group.size * m_ * n_ * 2, flops=2.0 * m_ * n_ * k_):
-            self.comm.gemm_reduce_scatter(group, a, b, m_, n_, k_, code, buf, buf.data_bytes, 3 * buf.data_bytes, out)
-        self.n_fused_gemm_rs = getattr(self, "n_fused_gemm_rs", 0) + 1
-        self.n_fused["gemm_rs"] += 1
+            self.comm.gemm_reduce_scatter(group, a, b, m_, n_, k_, code, buf, buf.layout.partials, buf.layout.scatter_counters, out)
+        self._count("gemm_rs")
         return out
+
+    def gemm_all_reduce(self, a, b, layout, group):
+        """[M, N] = sum over ``group`` of A op B, on every member.  Fused (GEMM + C5/C6 in one operation): partial tiles go to
+        their owner's HBM, the owner's tile reducer sums them as they land and broadcasts the rows into every member's result."""
+        code, m_, n_, k_ = self._mnk(a, b, layout)
+        if not self.fuses("gemm_ar", m_, n_, k_, group):
+            staged, _ = self.staging_tensor(group, (m_, n_), a.dtype)
+            self.gemm(a, b, layout, out=staged)
+            return self.all_reduce(staged, group)
+        buf = self.staging(group, m_ * n_ * 2)
+        lay = buf.layout
+        with self._timed("gemm_all_reduce", 2.0 * (group.size - 1) / group.size * m_ * n_ * 2, flops=2.0 * m_ * n_ * k_):
+            self.comm.gemm_all_reduce(group, a, b, m_, n_, k_, code, buf, lay.partials, lay.scatter_counters, lay.result)
+        self._count("gemm_ar")
+        # the symmetric result buffer is rewritten by the next fused all-reduce of this group: hand out a private copy
+        return buf.u8[lay.result: lay.result + m_ * n_ * 2].view(torch.bfloat16).view(m_, n_).clone()
+
+    def all_gather_gemm(self, a_local, b, layout, group):
+        """out[M, N] = gather_rows(a_local[M/p, K]) op B, layout 'tn' or 'nn'.  Returns (out, gathered A): on both paths the
+        gathered operand sits complete in region 0 of the group's staging buffer afterwards (the wgrad GEMM of the same layer reads
+        it there).  Fused (C7 + GEMM in one operation): the GEMM consumes the gathered blocks as they land."""
+        assert layout != "nt", "all_gather_gemm gathers the rows of A[M, K]"
+        p = group.size
+        code, ml, n_, k_ = self._mnk(a_local, b, layout)
+        m_ = ml * p
+        if not self.fuses("ag_gemm", m_, n_, k_, group):
+            gathered = self.all_gather_into_staging(a_local, group)
+            return self.gemm(gathered, b, layout), gathered
+        buf = self.staging(group, m_ * k_ * 2)
+        out = torch.empty(m_, n_, dtype=torch.bfloat16, device=a_local.device)
+        with self._timed("all_gather_gemm", (p - 1) / p * m_ * k_ * 2, flops=2.0 * m_ * n_ * k_):
+            self.comm.all_gather_gemm(group, a_local, b, out, m_, n_, k_, code, buf, 0, buf.layout.gather_counters, self.comm_stream)
+        a_local.record_stream(self.comm_stream)
+        self._count("ag_gemm")
+        return out, buf.u8[: m_ * k_ * 2].view(torch.bfloat16).view(m_, k_)
 
     def rmsnorm_fwd(self, x, weight, eps):
         x2 = x.reshape(-1, x.shape[-1])

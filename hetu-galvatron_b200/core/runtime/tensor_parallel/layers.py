@@ -63,11 +63,6 @@ def _write_wgrad(weight, dy2d, x2d):
     return None
 
 
-def _can(be, name, *args):
-    fn = getattr(be, name, None)
-    return bool(fn and fn(*args))
-
-
 class LinearWithGradAccumulationAndAsyncCommunication(torch.autograd.Function):
     """y = x W^T with the tensor/sequence-parallel communication of layers.py:375-547.
 
@@ -81,11 +76,12 @@ class LinearWithGradAccumulationAndAsyncCommunication(torch.autograd.Function):
         from -- ("swiglu", gate_up) or ("rmsnorm", x, norm_weight, eps), tensors the producing op keeps anyway -- and redo that
         elementwise pass in backward: one layer then holds 352 MiB less at Llama-3-8B / seq 8192.
 
-    Every GEMM that has a collective next to it runs as ONE fused operation when the shapes allow (M a multiple of p x 128):
+    Every GEMM that has a collective next to it is one backend operation, which runs as ONE fused kernel pair when the shapes allow
+    (M a multiple of p x 128) and otherwise writes the GEMM into the group's peer-visible staging buffer and runs the stand-alone
+    collective kernel after it:
       all-gather -> GEMM        ``backend.all_gather_gemm``      (C7: SP forward; the row-parallel dgrad under SP)
       GEMM -> reduce-scatter    ``backend.gemm_reduce_scatter``  (C8: row-parallel forward under SP; the SP dgrad)
       GEMM -> all-reduce        ``backend.gemm_all_reduce``      (C5: row-parallel forward; C6: column-parallel dgrad)
-    otherwise the GEMM writes into the group's peer-visible staging buffer and the stand-alone collective kernel follows.
     """
 
     @staticmethod
@@ -108,12 +104,7 @@ class LinearWithGradAccumulationAndAsyncCommunication(torch.autograd.Function):
             # row-parallel forward under Megatron-SP (layers.py:1061-1109): GEMM + reduce-scatter along the sequence
             ctx.sequence_parallel, ctx.allreduce_dgrad = False, False
             x2d = input.reshape(-1, input.shape[-1])
-            if _can(be, "can_fuse_gemm_rs", x2d.shape[0], n_out, tp_group, x2d.shape[1]):
-                out = be.gemm_reduce_scatter(x2d, weight, "tn", tp_group)       # one fused operation
-            else:
-                staged, _ = be.staging_tensor(tp_group, (x2d.shape[0], n_out), input.dtype)
-                be.gemm(x2d, weight, "tn", out=staged)
-                out = be.reduce_scatter_first_dim(staged, tp_group)
+            out = be.gemm_reduce_scatter(x2d, weight, "tn", tp_group)
             out = out.view(input.shape[0] // tp_group.size, *input.shape[1:-1], n_out)
             return out if addend is None else out + addend
         ctx.sequence_parallel = sequence_parallel and multi
@@ -121,22 +112,12 @@ class LinearWithGradAccumulationAndAsyncCommunication(torch.autograd.Function):
         if ctx.sequence_parallel:
             x2d = input.reshape(-1, input.shape[-1])
             full_shape = (input.shape[0] * tp_group.size,) + tuple(input.shape[1:-1])
-            if _can(be, "can_fuse_ag_gemm", x2d.shape[0] * tp_group.size, x2d.shape[1], tp_group):
-                out, _ = be.all_gather_gemm(x2d.contiguous(), weight, "tn", tp_group)   # gather and GEMM overlap block by block
-            else:
-                total = be.all_gather_into_staging(input, tp_group)
-                out = be.gemm(total.reshape(-1, total.shape[-1]), weight, "tn")
+            out, _ = be.all_gather_gemm(x2d.contiguous(), weight, "tn", tp_group)
             out = out.view(*full_shape, n_out)
             return out if addend is None else out + addend
         x2d = input.reshape(-1, input.shape[-1])
         if allreduce_out and multi:
-            if _can(be, "can_fuse_gemm_ar", x2d.shape[0], n_out, tp_group, x2d.shape[1]):
-                out = be.gemm_all_reduce(x2d, weight, "tn", tp_group)            # GEMM + two-shot all-reduce, one operation
-            else:
-                staged, _ = be.staging_tensor(tp_group, (x2d.shape[0], n_out), input.dtype)
-                be.gemm(x2d, weight, "tn", out=staged)
-                out = be.all_reduce(staged, tp_group)
-            out = out.view(*input.shape[:-1], n_out)
+            out = be.gemm_all_reduce(x2d, weight, "tn", tp_group).view(*input.shape[:-1], n_out)
             return out if addend is None else out + addend
         if addend is not None:
             return be.gemm(x2d, weight, "tn", addend=addend.contiguous().reshape(-1, n_out)).view(*input.shape[:-1], n_out)
@@ -165,7 +146,7 @@ class LinearWithGradAccumulationAndAsyncCommunication(torch.autograd.Function):
             # backward of the reduce-scatter is an all-gather along the sequence (mappings_group.py:243-258); the dgrad GEMM
             # consumes the gathered dy block by block while it arrives, and the wgrad GEMM reads it from staging afterwards
             dy_local = grad_output.reshape(-1, grad_output.shape[-1])
-            if ctx.needs_input_grad[0] and _can(be, "can_fuse_ag_gemm", dy_local.shape[0] * group.size, dy_local.shape[1], group):
+            if ctx.needs_input_grad[0] and be.fuses("ag_gemm", dy_local.shape[0] * group.size, k, dy_local.shape[1], group):
                 gi, dy2d = be.all_gather_gemm(dy_local.contiguous(), weight, "nn", group)
                 grad_input = gi.view(grad_output.shape[0] * group.size, *grad_output.shape[1:-1], k)
                 dgrad_done = True
@@ -176,11 +157,9 @@ class LinearWithGradAccumulationAndAsyncCommunication(torch.autograd.Function):
             dy2d = grad_output.reshape(-1, grad_output.shape[-1])
         if not dy2d.is_contiguous():
             dy2d = dy2d.contiguous()
-        m = dy2d.shape[0]
-        fuse_rs = ctx.sequence_parallel and ctx.needs_input_grad[0] and _can(be, "can_fuse_gemm_rs", m, k, group, dy2d.shape[1])
         total = input
         if weight.requires_grad and ctx.sequence_parallel:
-            if fuse_rs and getattr(be, "comm_stream", None) is not None:
+            if ctx.needs_input_grad[0] and be.fuses("gemm_rs", dy2d.shape[0], k, dy2d.shape[1], group):
                 # the re-gather of the input (for wgrad) runs on the communication stream WHILE the fused dgrad GEMM +
                 # reduce-scatter runs here (layers.py:449-462 overlaps the same pair); wgrad waits for it below
                 total, gather_event = be.all_gather_into_staging(input, group, overlap=True)
@@ -190,20 +169,12 @@ class LinearWithGradAccumulationAndAsyncCommunication(torch.autograd.Function):
         if weight.requires_grad and gather_event is None:
             grad_weight = _write_wgrad(weight, dy2d, total.reshape(-1, total.shape[-1]))
         if ctx.needs_input_grad[0] and not dgrad_done:
-            if fuse_rs:
-                # dgrad GEMM + reduce-scatter along the sequence (layers.py:462,488-494) as one fused operation
+            if ctx.sequence_parallel:
+                # dgrad GEMM + reduce-scatter along the sequence (layers.py:462,488-494)
                 out = be.gemm_reduce_scatter(dy2d, weight, "nn", group)
                 grad_input = out.view(grad_output.shape[0] // group.size, *grad_output.shape[1:-1], k)
-            elif ctx.allreduce_dgrad and _can(be, "can_fuse_gemm_ar", m, k, group, dy2d.shape[1]):
+            elif ctx.allreduce_dgrad:
                 grad_input = be.gemm_all_reduce(dy2d, weight, "nn", group).view(*grad_output.shape[:-1], k)
-            elif ctx.sequence_parallel or ctx.allreduce_dgrad:
-                staged, _ = be.staging_tensor(group, (m, k), dy2d.dtype)  # overwrites the gathered input: wgrad is done
-                be.gemm(dy2d, weight, "nn", out=staged)
-                full_shape = grad_output.shape[:-1] + (k,)
-                if ctx.sequence_parallel:
-                    grad_input = be.reduce_scatter_first_dim(staged.view(*full_shape), group)
-                else:
-                    grad_input = be.all_reduce(staged.view(*full_shape), group)
             else:
                 grad_input = be.gemm(dy2d, weight, "nn").view(*grad_output.shape[:-1], k)
         if gather_event is not None:

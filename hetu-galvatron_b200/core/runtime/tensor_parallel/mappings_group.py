@@ -87,13 +87,6 @@ class _ReduceFromModelParallelRegion(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, input_, group):
-        # (opt-in, HGB_NVLS=1 + HGB_NVLS_INPLACE=1) a GEMM output that already lives in the group's multicast-bound staging buffer is
-        # reduced inside the NVSwitch and handed on in place: no copy-out.  Its consumer (the residual add) reads it before the
-        # next GEMM of this rank is launched into the same buffer.
-        inplace = getattr(get_backend(), "all_reduce_inplace", None)
-        if inplace is not None and _size(group) > 1 and inplace(input_, group):
-            ctx.mark_dirty(input_)
-            return input_
         return _reduce(input_, group)
 
     @staticmethod

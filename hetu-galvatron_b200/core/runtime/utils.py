@@ -365,11 +365,10 @@ def clip_grad_norm(model, max_norm, norm_type=2):
     buf = torch.zeros(8, dtype=torch.float32, device=device)
     buf[0] = total
     if be.world > 1:
-        world_group = getattr(be, "world_group", None)
-        if world_group is None:
+        if be.world_group is None:
             raise RuntimeError("clip_grad_norm over %d ranks needs the world group reserved at model construction "
                                "(construct_hybrid_parallel_model_api does it; worlds beyond one NVSwitch domain are out of scope)" % be.world)
-        buf = be.all_reduce(buf, world_group)
+        buf = be.all_reduce(buf, be.world_group)
     norm = buf[0].sqrt()
     coef = (max_norm / (norm + 1e-6)).clamp(max=1.0)
     for g in grads:

@@ -1016,33 +1016,6 @@ extern "C" int bg_all_to_all_rows(bg_ctx_t c, int gid, int lane, const bg_a2a_de
     return BG_OK;
 }
 
-// In-switch all-reduce on an explicit range of the group's multicast-bound region (kept for callers that manage the buffer
-// themselves; bg_all_reduce picks the same kernel on its own when its source is multicast-addressable).
-extern "C" int bg_all_reduce_nvls(bg_ctx_t c, int gid, int lane, size_t byte_offset, void* dst, size_t elems, int dtype, float scale,
-                                  void* stream) {
-    Sig s; const Group* g;
-    int rc = make_sig(c, gid, lane, &s, &g);
-    if (rc) return rc;
-    auto it = c->mc_of.find(gid);
-    if (it == c->mc_of.end() || !it->second.bound) return fail(BG_EINVAL, "group %d has no bound NVLS buffer", gid);
-    const bg_ctx::McGroup& m = it->second;
-    const size_t esz = dtype == BG_BF16 ? 2 : dtype == BG_F32 ? 4 : 0;
-    if (!esz) return fail(BG_EUNSUPPORTED, "bg_all_reduce_nvls: bf16 or fp32");
-    if (elems * esz % 16) return fail(BG_EINVAL, "bg_all_reduce_nvls: payload must be a multiple of 16 bytes");
-    if (byte_offset % 16 || byte_offset + elems * esz > m.bytes)
-        return fail(BG_EINVAL, "bg_all_reduce_nvls: [%zu,+%zu) outside the bound buffer (%zu B) or misaligned", byte_offset, elems * esz, m.bytes);
-    BG_CUDA(cudaSetDevice(c->device));
-    const size_t vecs = elems * esz / 16;
-    const int grid = comm_grid((vecs + g->n - 1) / g->n / kInFlight + 1, kThreads, g->n);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (dtype == BG_BF16)
-        all_reduce_nvls_kernel<true><<<grid, kThreads, 0, st>>>((char*)m.va + byte_offset, c->arena + m.arena_off + byte_offset, (char*)dst, vecs, scale, s);
-    else
-        all_reduce_nvls_kernel<false><<<grid, kThreads, 0, st>>>((char*)m.va + byte_offset, c->arena + m.arena_off + byte_offset, (char*)dst, vecs, scale, s);
-    BG_CHECK_LAUNCH();
-    return BG_OK;
-}
-
 // ------------------------------------------------------------------------------------------------
 // C15: ring context parallelism
 // ------------------------------------------------------------------------------------------------

@@ -749,7 +749,8 @@ int bg_gemm_scatter_launch(const void* a, const void* b, long long m, long long 
         for (int i = 0; i < p; ++i) bc.out[i] = (char*)bcast_ptrs[i];
     }
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)rgrid); cfg.blockDim = dim3(128);   // slim: fits beside the GEMM CTA and two more collectives cfg.dynamicSmemBytes = 0; cfg.stream = st;
+    cfg.gridDim = dim3((unsigned)rgrid); cfg.blockDim = dim3(128);   // slim: fits beside the GEMM CTA and two more collectives
+    cfg.dynamicSmemBytes = 0; cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;

@@ -303,8 +303,7 @@ int bg_all_gather_gemm(bg_ctx_t ctx, int gid, int lane, const void* a_local, con
  * Replaces the tensor-parallel all-reduces (mappings_group.py:19, layers.py:474-480) for large messages, where NCCL itself
  * switches to NVLS: N/p bytes in and N/p out per GPU instead of 2(p-1)/p*N.  One multicast object per group over one
  * symmetric buffer: the group's first rank creates it (-> fd), every other member imports the fd, ALL join (device added),
- * barrier on the host, ALL bind their own arena range (multicast-granularity aligned), then bg_all_reduce_nvls works in
- * place on that buffer and copies the result to dst (dst may be NULL: result left in the buffer).  BG_CTX_VMM contexts only.
+ * barrier on the host, ALL bind their own arena range (multicast-granularity aligned).  BG_CTX_VMM contexts only.
  * The bound range may be any part of the arena (the host binds the whole region that holds its symmetric buffers): every
  * collective whose buffer lies inside it at the same offset on all members then uses the switch on its own --
  * bg_all_reduce (ld_reduce + st), bg_all_gather_cast and the bg_gemm_all_reduce broadcast (multimem.st), bg_reduce_scatter_acc /
@@ -313,8 +312,6 @@ int bg_group_mc_create(bg_ctx_t ctx, int gid, size_t bytes, int* fd_out);
 int bg_group_mc_join(bg_ctx_t ctx, int gid, int fd /* -1 on the creator */, size_t bytes);
 int bg_group_mc_bind(bg_ctx_t ctx, int gid, size_t arena_offset);
 int bg_group_mc_disable(bg_ctx_t ctx, int gid);   /* setup failed on some member: the group keeps the peer-to-peer kernels */
-int bg_all_reduce_nvls(bg_ctx_t ctx, int gid, int lane, size_t byte_offset, void* dst, size_t elems, int dtype, float scale,
-                       void* stream);
 
 #ifdef __cplusplus
 }

@@ -65,6 +65,7 @@ class OracleBackend:
         self.world = dist.get_world_size() if dist.is_initialized() else 1
         self._pgs = {}
         self._staging = {}
+        self.world_group = None
         if self.world > 1:
             # every arithmetic-progression subgroup, created in the same order on all ranks (new_group is collective)
             for stride in range(1, self.world):
@@ -89,9 +90,6 @@ class OracleBackend:
 
     def reserve_staging(self, group, nbytes):
         return None
-
-    def staging_tensor(self, group, shape, dtype, byte_offset=0):
-        return torch.empty(*shape, dtype=dtype), None
 
     # ---- sharded units ---------------------------------------------------------------------------------------------------
     def begin_step(self):
@@ -213,8 +211,22 @@ class OracleBackend:
                 outs.append(torch.cat([allt[q][:, r * sl:(r + 1) * sl] for q in range(p)], dim=2).contiguous())
         return outs
 
+    # ---- GEMM + collective: the GEMM, then the collective (megatron/core/tensor_parallel/layers.py:399-417, :462, :488-494) ---------
+    def fuses(self, kind, m, n, k, group):
+        return False
+
+    def gemm_reduce_scatter(self, a, b, layout, group):
+        return self.reduce_scatter_first_dim(self.gemm(a, b, layout), group)
+
+    def gemm_all_reduce(self, a, b, layout, group):
+        return self.all_reduce(self.gemm(a, b, layout), group)
+
+    def all_gather_gemm(self, a_local, b, layout, group):
+        gathered = self.all_gather_first_dim(a_local, group)
+        return self.gemm(gathered, b, layout), gathered
+
     # ---- math -------------------------------------------------------------------------------------------------------------------
-    def gemm(self, a, b, layout, out=None, accumulate=False, m=None, n=None, k=None, addend=None):
+    def gemm(self, a, b, layout, out=None, accumulate=False, addend=None):
         self.launches += 1
         af = a.float().t() if layout == "nt" else a.float()
         bf = b.float().t() if layout == "tn" else b.float()

@@ -265,7 +265,7 @@ def main():
                        for k, p in getattr(be, "_zero3_pools", {}).items()}
     if use_cuda:
         report["launches"] = be.launch_count()
-        report["fused_gemm_rs_calls"] = getattr(be, "n_fused_gemm_rs", 0)
+        report["fused_gemm_rs_calls"] = be.n_fused["gemm_rs"]
         report["fused_calls"] = dict(getattr(be, "n_fused", {}))
     if rank == 0:
         print("HOST_TEST_REPORT " + json.dumps(report), flush=True)
