@@ -5,11 +5,31 @@ import torch.nn as nn
 from ..core.runtime.arguments import get_args
 from ..core.runtime.hybrid_parallel_config import ModelInfo, mixed_precision_dtype
 from ..core.runtime.pipeline import PipeSequential
-from ..core.runtime.tensor_parallel import (gather_from_tensor_model_parallel_region_group,
+from ..core.runtime.tensor_parallel import (VocabUtility, gather_from_tensor_model_parallel_region_group,
                                             linear_with_grad_accumulation_and_async_allreduce,
                                             scatter_to_sequence_parallel_region_group, vocab_parallel_cross_entropy)
-from ..core.runtime.tensor_parallel.random import check_probability
-from ..gpt_hf.GPTModel_sequential import _embedding_dropout, _seq_slice, _size
+from ..core.runtime.tensor_parallel.random import SITE_EMBEDDING, bias_dropout_add, check_probability, site
+
+
+def _size(g):
+    return 1 if g is None else g.size
+
+
+def _embedding_dropout(module, hidden_states):
+    """Embedding dropout (hidden_dropout) on the SBH slice this rank holds after the vocab_sp slice and the Megatron-SP scatter, at
+    global token positions."""
+    if not (module.dropout_p > 0.0 and module.training):
+        return hidden_states
+    seq_base = module.seq_start_index if module.vocab_sp else 0
+    if module.sequence_parallel and _size(module.tp_group) > 1:
+        seq_base += module.tp_group.rank_in_group() * hidden_states.shape[0]
+    return bias_dropout_add(hidden_states, None, None, module.dropout_p, site(0, SITE_EMBEDDING), seq_base)
+
+
+def _seq_slice(args, sp_group):
+    """Ulysses on the vocabulary rows: each rank embeds / scores its own sequence slice (:59-64,159-165)."""
+    return VocabUtility.vocab_range_from_global_vocab_size(args.seq_length, sp_group.rank_in_group() if _size(sp_group) > 1 else 0,
+                                                           _size(sp_group))
 
 
 class BertWordEmbedding_(nn.Module):

@@ -60,6 +60,32 @@ def local_positions(seq, cp=1, cp_rank=0, sp=1, sp_rank=0):
     return idx[sp_rank * n:(sp_rank + 1) * n]
 
 
+def zigzag_local(x, group, sp_group=None):
+    """[b, s] tokens / labels / positions -> the tokens this rank holds [b, s/(c*p)]: the context-parallel rank's two zigzag chunks
+    (r, 2c-1-r), and of those the Ulysses rank's contiguous slice (``local_positions``).  The reference's real-data loader does this
+    slicing before the model (Megatron ``get_batch_on_this_cp_rank``, models/llama_hf/dataloader.py:151, then the vocab_sp slice
+    :45-57); here the first and the last layer do it, so ``forward_backward`` takes the same full-sequence batch in every mode."""
+    c, p = _size(group), _size(sp_group)
+    if c == 1 and p == 1:
+        return x
+    idx = local_positions(x.shape[1], c, group.rank_in_group() if c > 1 else 0, p, sp_group.rank_in_group() if p > 1 else 0)
+    if c == 1:      # one contiguous slice
+        return x[:, int(idx[0]):int(idx[-1]) + 1].contiguous()
+    return x[:, idx.to(x.device)].contiguous()
+
+
+def token_runs(positions):
+    """Global token positions of a rank's rows (row order) -> the maximal runs of consecutive tokens, ((first row, rows, first
+    token), ...).  A zigzag rank's rows are at most two runs, and so is any contiguous slice of them (Megatron-SP, Ulysses)."""
+    pos = [int(t) for t in positions]
+    runs, start = [], 0
+    for i in range(1, len(pos) + 1):
+        if i == len(pos) or pos[i] != pos[i - 1] + 1:
+            runs.append((start, i - start, pos[start]))
+            start = i
+    return tuple(runs)
+
+
 def _reverse_zigzag_transformation(x, cp):
     if cp == 1:
         return x

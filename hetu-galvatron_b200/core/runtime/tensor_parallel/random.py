@@ -65,28 +65,46 @@ def set_context(ctx):
 
 
 class _BiasDropoutAddFn(torch.autograd.Function):
-    """y = residual + keep * scale * (x + bias): one row kernel forward, one backward that regenerates the mask."""
+    """y = residual + keep * scale * (x + bias): one row kernel forward, one backward that regenerates the mask -- one launch of
+    each per run of consecutive tokens in the local rows (a zigzag context-parallel rank holds two runs)."""
 
     @staticmethod
-    def forward(ctx, x, bias, residual, p, coords):
-        ctx.p, ctx.coords = p, coords            # (seed, iteration, site, seq_base, sample_base): plain integers, no global state
+    def forward(ctx, x, bias, residual, p, coords, runs):
+        ctx.p, ctx.coords, ctx.runs = p, coords, runs     # (seed, iteration, site, sample_base), ((row0, rows, token0), ...)
         ctx.has_residual, ctx.bias_dtype = residual is not None, None if bias is None else bias.dtype
-        return get_backend().dropout_add_fwd(x, bias, residual, p, *coords)
+        seed, iteration, site_id, sample_base = coords
+        be = get_backend()
+        if len(runs) == 1:
+            return be.dropout_add_fwd(x, bias, residual, p, seed, iteration, site_id, runs[0][2], sample_base)
+        return torch.cat([be.dropout_add_fwd(x[r0:r0 + n], bias, None if residual is None else residual[r0:r0 + n], p, seed, iteration,
+                                             site_id, t0, sample_base) for r0, n, t0 in runs])
 
     @staticmethod
     def backward(ctx, dy):
-        dx, db = get_backend().dropout_bwd(dy, ctx.p, *ctx.coords, with_bias=ctx.bias_dtype is not None)
-        return dx, (None if db is None else db.to(ctx.bias_dtype)), (dy if ctx.has_residual else None), None, None
+        seed, iteration, site_id, sample_base = ctx.coords
+        with_bias, be = ctx.bias_dtype is not None, get_backend()
+        parts = [be.dropout_bwd(dy[r0:r0 + n], ctx.p, seed, iteration, site_id, t0, sample_base, with_bias=with_bias)
+                 for r0, n, t0 in ctx.runs]
+        dx = parts[0][0] if len(parts) == 1 else torch.cat([d for d, _ in parts])
+        db = None if not with_bias else (parts[0][1] if len(parts) == 1 else sum(b for _, b in parts)).to(ctx.bias_dtype)
+        return dx, db, (dy if ctx.has_residual else None), None, None, None
 
 
 def bias_dropout_add(x, bias, residual, p, site_id, seq_base=0):
-    """Dropout of an SBH tensor x [s_loc, b_loc, h] (plus bias, plus residual) with the current microbatch's dropout context; the
-    local rows are tokens ``seq_base``.. of the microbatch's samples."""
+    """Dropout of an SBH tensor x [s_loc, b_loc, h] (plus bias, plus residual) with the current microbatch's dropout context.
+    ``seq_base``: the local rows are tokens ``seq_base``.. of the microbatch's samples; or the rows' runs of consecutive tokens,
+    ((first row, rows, first token), ...) as ``redistribute.token_runs`` gives them, covering the rows in order."""
     ctx = _CTX
     if ctx.batch is not None and x.shape[1] != ctx.batch:
         raise NotImplementedError("dropout: a layer sees %d samples of a %d-sample microbatch (a relocation that re-splits the batch "
                                   "is not supported with dropout)" % (x.shape[1], ctx.batch))
-    return _BiasDropoutAddFn.apply(x, bias, residual, float(p), (ctx.seed, ctx.iteration, int(site_id), int(seq_base), ctx.sample_base))
+    if isinstance(seq_base, (tuple, list)):
+        runs = tuple(tuple(int(v) for v in run) for run in seq_base)
+    else:
+        runs = ((0, x.shape[0], int(seq_base)),)
+    if runs[0][0] != 0 or sum(n for _, n, _ in runs) != x.shape[0] or any(a[0] + a[1] != b[0] for a, b in zip(runs, runs[1:])):
+        raise ValueError("dropout: token runs %s do not cover the %d local rows in order" % (runs, x.shape[0]))
+    return _BiasDropoutAddFn.apply(x, bias, residual, float(p), (ctx.seed, ctx.iteration, int(site_id), ctx.sample_base), runs)
 
 
 class RngTracker:

@@ -5,31 +5,15 @@ import torch.nn as nn
 from ..core.runtime.arguments import get_args
 from ..core.runtime.hybrid_parallel_config import ModelInfo, mixed_precision_dtype
 from ..core.runtime.pipeline import PipeSequential
-from ..core.runtime.tensor_parallel import (VocabUtility, gather_from_tensor_model_parallel_region_group,
-                                            linear_with_grad_accumulation_and_async_allreduce,
+from ..core.runtime.redistribute import zigzag_local
+from ..core.runtime.tensor_parallel import (gather_from_tensor_model_parallel_region_group, linear_with_grad_accumulation_and_async_allreduce,
                                             scatter_to_sequence_parallel_region_group, vocab_parallel_cross_entropy)
 from ..core.runtime.tensor_parallel.random import SITE_EMBEDDING, bias_dropout_add, check_probability, site
+from .GPTModel_tensor_parallel import row_runs
 
 
 def _size(g):
     return 1 if g is None else g.size
-
-
-def _embedding_dropout(module, hidden_states):
-    """Embedding dropout (hidden_dropout) on the SBH slice this rank holds after the vocab_sp slice and the Megatron-SP scatter, at
-    global token positions."""
-    if not (module.dropout_p > 0.0 and module.training):
-        return hidden_states
-    seq_base = module.seq_start_index if module.vocab_sp else 0
-    if module.sequence_parallel and _size(module.tp_group) > 1:
-        seq_base += module.tp_group.rank_in_group() * hidden_states.shape[0]
-    return bias_dropout_add(hidden_states, None, None, module.dropout_p, site(0, SITE_EMBEDDING), seq_base)
-
-
-def _seq_slice(args, sp_group):
-    """Ulysses on the vocabulary rows: each rank embeds / scores its own sequence slice (:59-64,159-165)."""
-    return VocabUtility.vocab_range_from_global_vocab_size(args.seq_length, sp_group.rank_in_group() if _size(sp_group) > 1 else 0,
-                                                           _size(sp_group))
 
 
 class GPTVocabEmbedding_(nn.Module):
@@ -56,23 +40,34 @@ class GPTEmbeddings_(nn.Module):
         args = get_args()
         self.wte, self.wpe = GPTVocabEmbedding_(model.transformer), GPTPositionEmbedding_(model.transformer)
         self.sequence_parallel = args.sequence_parallel
-        self.tp_group, self.sp_group = self.wte.wte.tp_group, self.wte.wte.sp_group
-        self.vocab_sp = args.vocab_sp
-        if self.vocab_sp:
-            self.seq_start_index, self.seq_end_index = _seq_slice(args, self.sp_group)
+        self.tp_group, self.sp_group, self.cp_group = self.wte.wte.tp_group, self.wte.wte.sp_group, self.wte.wte.cp_group
+        # Ulysses on the embedding: each rank embeds its own sequence slice (:59-64), of the cp rank's zigzag chunks under cp
+        self.seq_group = self.sp_group if args.vocab_sp else None
         self.dropout_p = check_probability(getattr(args, "hidden_dropout", 0.0), "hidden_dropout")     # :55
+        self.tp_split = self.tp_group if self.sequence_parallel and _size(self.tp_group) > 1 else None
+        self._runs = {}
+        c, p = _size(self.cp_group), _size(self.seq_group)
+        if c > 1 and args.seq_length % (2 * c * p):
+            raise ValueError("GPT with context parallelism: sequence length %d must be a multiple of 2 x cp%s = %d"
+                             % (args.seq_length, " x sp" if p > 1 else "", 2 * c * p))
 
     def forward(self, tokens, position_ids=None, attention_mask=None, labels=None):
         if position_ids is None:
             position_ids = torch.arange(0, tokens.size(-1), dtype=torch.long, device=tokens.device).unsqueeze(0)
-        if self.vocab_sp:
-            tokens = tokens[:, self.seq_start_index:self.seq_end_index].contiguous()
-            position_ids = position_ids[:, self.seq_start_index:self.seq_end_index].contiguous()
+        # this rank's tokens and their GLOBAL positions: the learned position table is looked up where the tokens sit in the sequence
+        tokens = zigzag_local(tokens, self.cp_group, self.seq_group)
+        position_ids = zigzag_local(position_ids, self.cp_group, self.seq_group)
         hidden_states = self.wte(tokens) + self.wpe(position_ids)
         hidden_states = hidden_states.transpose(0, 1).contiguous()           # [b, s, h] -> [s, b, h]
         if self.sequence_parallel:
             hidden_states = scatter_to_sequence_parallel_region_group(hidden_states, self.tp_group)
-        return _embedding_dropout(self, hidden_states)
+        if not (self.dropout_p > 0.0 and self.training):
+            return hidden_states
+        # embedding dropout (hidden_dropout) on the rows this rank holds after the Megatron-SP scatter, at their global token positions
+        rows = hidden_states.shape[0]
+        if rows not in self._runs:
+            self._runs[rows] = row_runs(rows, self.cp_group, self.seq_group, self.tp_split)
+        return bias_dropout_add(hidden_states, None, None, self.dropout_p, site(0, SITE_EMBEDDING), self._runs[rows])
 
 
 class GPTLayers_(nn.Module):
@@ -117,17 +112,16 @@ class GPTCls_(nn.Module):
         super().__init__()
         args = get_args()
         self.sequence_parallel = args.sequence_parallel
-        self.tp_group, self.sp_group = model.lm_head.tp_group, model.lm_head.sp_group
-        self.lm_head = GPTLoss_(model.lm_head, self.sequence_parallel, self.tp_group)
+        head = model.lm_head
+        self.tp_group, self.sp_group, self.cp_group = head.tp_group, head.sp_group, head.cp_group
+        self.lm_head = GPTLoss_(head, self.sequence_parallel, self.tp_group)
         self.parallel_loss = parallel_loss
         self.half_entropy = half_entropy and not args.entropy_in_fp32
         self.vocab_sp = args.vocab_sp
-        if self.vocab_sp:
-            self.seq_start_index, self.seq_end_index = _seq_slice(args, self.sp_group)
+        self.seq_group = self.sp_group if self.vocab_sp else None
 
     def forward(self, hidden_states, position_ids=None, attention_mask=None, labels=None):
-        if self.vocab_sp:
-            labels = labels[:, self.seq_start_index:self.seq_end_index].contiguous()
+        labels = zigzag_local(labels, self.cp_group, self.seq_group)
         logits_parallel = self.lm_head(hidden_states)                          # [s, b, V/t]
         labels = labels.transpose(0, 1).contiguous()                            # [b, s] -> [s, b]
         if not self.parallel_loss:

@@ -71,7 +71,26 @@ def estimate_arena_bytes(config, args, hp_configs):
     mbs = -(-args.global_train_batch_size // min_dp // max(1, args.chunks if args.chunks > 0 else 1))
     act = int(config.max_position_embeddings * mbs * h * esz * 1.5) + (1 << 20)
     n_groups = 0 if world == 1 else 8
-    return int(total * 1.02) + act * n_groups + 4 * act + (64 << 20)
+    return int(total * 1.02) + act * n_groups + 4 * act + _cp_ring_bytes(config, args, hp_configs, mbs) + (64 << 20)
+
+
+def _cp_ring_bytes(config, args, hp_configs, mbs):
+    """cp_comm="ring": the receive slots hybrid_parallel_model reserves per cp group, 24 B per element of the largest local K block
+    (microbatch x s/c x K/V heads at the attention call x head dim) -- for MHA (GPT) four times the activation staging of a group at
+    c = 2.  Summed over the distinct (tp|sp, cp) layer strategies, each of which may have a cp group of its own."""
+    from ..core.runtime.tensor_parallel.transformer import cp_comm_mode
+    if cp_comm_mode() != "ring":
+        return 0
+    n, ng = config.num_attention_heads, config.num_key_value_heads
+    hn, seq = config.hidden_size // n, config.max_position_embeddings
+    use_sp = hp_configs.get("use_sp") or [0] * len(hp_configs["tp_sizes_enc"])
+    total = 0
+    for deg, cp, sp in set(zip(hp_configs["tp_sizes_enc"], hp_configs["cp_sizes_enc"], use_sp)):
+        if cp > 1:
+            # ParallelAttention.kv_heads_attn: Ulysses (degree ``deg``) leaves ng/p heads, or n/p when K/V are replicated first
+            kv = ((ng if ng % deg == 0 else n) // deg) if sp else ng // deg
+            total += 24 * mbs * (seq // cp) * kv * hn
+    return total
 
 
 def llama_model_hp(config, args):

@@ -5,7 +5,7 @@ import torch.nn as nn
 from ..core.runtime.arguments import get_args
 from ..core.runtime.hybrid_parallel_config import ModelInfo, mixed_precision_dtype
 from ..core.runtime.pipeline import PipeSequential
-from ..core.runtime.redistribute import local_positions
+from ..core.runtime.redistribute import zigzag_local as _zigzag_local
 from ..core.runtime.tensor_parallel import (RMSNorm, copy_to_tensor_model_parallel_region_group,
                                             gather_from_tensor_model_parallel_region_group,
                                             linear_with_grad_accumulation_and_async_allreduce,
@@ -14,21 +14,6 @@ from ..core.runtime.tensor_parallel import (RMSNorm, copy_to_tensor_model_parall
 
 def _size(g):
     return 1 if g is None else g.size
-
-
-def _zigzag_local(x, group, sp_group=None):
-    """[b, s] tokens / labels -> the tokens this rank holds [b, s/(c*p)]: the context-parallel rank's two zigzag chunks
-    (r, 2c-1-r), and of those the Ulysses rank's contiguous slice (redistribute.local_positions).  The reference's real-data
-    loader does this slicing before the model (Megatron ``get_batch_on_this_cp_rank``, models/llama_hf/dataloader.py:151,
-    then the vocab_sp slice :45-57); here the first and the last layer do it, so ``forward_backward`` takes the same
-    full-sequence batch in every mode."""
-    c, p = _size(group), _size(sp_group)
-    if c == 1 and p == 1:
-        return x
-    idx = local_positions(x.shape[1], c, group.rank_in_group() if c > 1 else 0, p, sp_group.rank_in_group() if p > 1 else 0)
-    if c == 1:      # one contiguous slice
-        return x[:, int(idx[0]):int(idx[-1]) + 1].contiguous()
-    return x[:, idx.to(x.device)].contiguous()
 
 
 class LlamaEmbeddings_(nn.Module):

@@ -1,5 +1,6 @@
 """Micro-benchmarks of the C-ABI kernels on one GPU (CUDA events, warm-up, L2-exceeding inputs).
-Usage: python scripts/bench_kernels.py [gemm] [cast] [ops] [attn] [dropout] [cp] [clip]  -> JSON lines on stdout."""
+Usage: python scripts/bench_kernels.py [gemm] [cast] [ops] [attn] [dropout] [cp] [clip]  -> JSON lines on stdout.
+       cp's head shape and sequence lengths: --cp-heads N --cp-kv-heads N --cp-head-dim N --cp-seqs S1,S2 (defaults: Llama-3.2-1B)."""
 import json
 import os
 import sys
@@ -314,8 +315,9 @@ class _LocalRing:
         pass
 
 
-def cp():
-    """Ring context parallelism at Llama-3.2-1B attention shapes (32 heads, 8 KV heads of 64), microbatch 1, sequence S in {32k, 128k},
+def cp(n=32, ng=8, d=64, seqs=(32768, 131072)):
+    """Ring context parallelism at Llama-3.2-1B attention shapes (32 heads, 8 KV heads of 64) by default, or the given heads / KV heads /
+    head dim (``--cp-heads 32 --cp-kv-heads 32 --cp-head-dim 128``: GPT-3 6.7B), microbatch 1, sequence S in {32k, 128k} (``--cp-seqs``),
     cp degree c in {2, 4, 8}.  Per rank: attention forward + backward of the ring schedule (2c-1 flash-attn block calls, the LSE
     merges and the fp32 accumulation casts; transport excluded) against the all-gather path's two prefix calls on the gathered
     sequence (gather excluded); the merge and the two push kernels in GB/s over algorithmic bytes -- the pushes between two virtual
@@ -327,10 +329,11 @@ def cp():
     from hetu_galvatron_b200.core.runtime.tensor_parallel import transformer as tr
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
     print(json.dumps({"nvidia_smi": q.stdout.strip()}), flush=True)
-    n, ng, d, b = 32, 8, 64, 1
+    b = 1
+    shape = {} if (n, ng, d) == (32, 8, 64) else {"heads": n, "kv_heads": ng, "head_dim": d}
     scale = d ** -0.5
     be = CudaBackend(arena_bytes=1 << 24)
-    for S in (32768, 131072):
+    for S in seqs:
         for c in (2, 4, 8):
             s = S // c
             qq = torch.randn(b, s, n, d, device="cuda").to(BF)
@@ -355,7 +358,7 @@ def cp():
                 t_ring.append(timeit(ring_fb, iters=iters, warm=1))
                 t_gather.append(timeit(gather_fb, iters=iters, warm=1))
             kv_ring, kv_gather = 2 * b * s * ng * d * 2, 2 * b * S * ng * d * 2
-            print(json.dumps({"bench": "cp_attention_fwd_bwd_per_rank", "S": S, "c": c, "ring_ms": round(sorted(t_ring)[1], 3),
+            print(json.dumps({"bench": "cp_attention_fwd_bwd_per_rank", **shape, "S": S, "c": c, "ring_ms": round(sorted(t_ring)[1], 3),
                               "gather_ms": round(sorted(t_gather)[1], 3), "ring_over_gather": round(sorted(t_ring)[1] / sorted(t_gather)[1], 3),
                               "spread_pct": round(100 * (max(t_ring + t_gather) - min(t_ring + t_gather)) / min(t_ring + t_gather), 1),
                               "transport": "excluded (both paths)", "kv_kept_for_backward_MiB_ring": round(kv_ring / 2 ** 20, 1),
@@ -452,7 +455,17 @@ def clip():
 
 
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["gemm", "cast"]
+    import argparse
+    ap = argparse.ArgumentParser(description="kernel micro-benchmarks; JSON lines on stdout")
+    ap.add_argument("which", nargs="*", default=["gemm", "cast"])
+    ap.add_argument("--cp-heads", type=int, default=32, help="cp: query heads")
+    ap.add_argument("--cp-kv-heads", type=int, default=8, help="cp: key/value heads")
+    ap.add_argument("--cp-head-dim", type=int, default=64, help="cp: head dimension")
+    ap.add_argument("--cp-seqs", default="32768,131072", help="cp: comma-separated sequence lengths")
+    opts = ap.parse_args()
     print(json.dumps({"device": torch.cuda.get_device_name(0)}))
-    for w in which:
-        globals()[w]()
+    for w in opts.which:
+        if w == "cp":
+            cp(opts.cp_heads, opts.cp_kv_heads, opts.cp_head_dim, tuple(int(x) for x in opts.cp_seqs.split(",")))
+        else:
+            globals()[w]()
