@@ -67,6 +67,7 @@ SIGNATURES = {
     "bg_all_gather_cast": (_i, [_vp, _i, _i, _vp, _i, _c.POINTER(_sz), _i, _sz, _vp]),
     "bg_reduce_scatter_acc": (_i, [_vp, _i, _i, _c.POINTER(_sz), _i, _vp, _i, _sz, _f, _f, _i, _vp]),
     "bg_all_reduce": (_i, [_vp, _i, _i, _c.POINTER(_sz), _vp, _sz, _i, _i, _f, _vp]),
+    "bg_pair_sum_inplace": (_i, [_vp, _i, _i, _c.POINTER(_sz), _sz, _i, _f, _vp]),
     "bg_reduce_scatter_adamw": (_i, [_vp, _i, _i, _c.POINTER(_sz), _i, _vp, _vp, _vp, _sz, _f, _f, _f, _f, _f, _f, _f, _ll, _vp]),
     "bg_reduce_scatter_sumsq": (_i, [_vp, _i, _i, _c.POINTER(_sz), _i, _vp, _sz, _f, _f, _vp, _i, _c.POINTER(_sz), _i, _vp]),
     "bg_reduce_scatter_adamw_clipped": (_i, [_vp, _i, _i, _c.POINTER(_sz), _i, _vp, _vp, _vp, _sz, _f, _f, _f, _f, _f, _f, _f, _ll, _vp,
@@ -177,10 +178,12 @@ class _ArenaExport:
 
 
 class SymBuffer:
-    """A symmetric buffer: one allocation per member of ``group`` (arena offsets differ per rank)."""
+    """A symmetric buffer: one allocation per member of ``group`` (arena offsets differ per rank).  ``registered``: a view of an
+    existing arena range (``BgComm.sym_register``) rather than an allocation of its own."""
 
-    def __init__(self, comm, group, nbytes, offset, tensor_u8, key):
+    def __init__(self, comm, group, nbytes, offset, tensor_u8, key, registered=False):
         self.comm, self.group, self.nbytes, self.offset, self.u8, self.key = comm, group, nbytes, offset, tensor_u8, key
+        self.registered = registered
         self.offsets = None  # ctypes size_t[group.size] once exchanged
 
     def view(self, dtype, numel=None):
@@ -344,7 +347,8 @@ class BgComm:
             return {}
         regions = {}
         for buf in self._sym.values():
-            if buf.group.size < 2 or buf.offsets is None or len(set(int(o) for o in buf.offsets)) != 1:
+            # (a registered range lies inside memory of another group -- a unit's gradient buffer: a bind over it would cover that)
+            if buf.registered or buf.group.size < 2 or buf.offsets is None or len(set(int(o) for o in buf.offsets)) != 1:
                 continue
             ranks = tuple(buf.group.ranks)
             lo, hi = regions.get(ranks, (1 << 62, 0))
@@ -432,27 +436,43 @@ class BgComm:
         per group (SPMD); peer offsets become known at the next ``exchange()``.  ``align``: offset AND size granularity
         (the multicast granularity for a buffer that NVLS binds)."""
         nbytes = (int(nbytes) + align - 1) // align * align
-        ranks = tuple(group.ranks)
-        seq = self._sym_seq.get(ranks, 0)
-        self._sym_seq[ranks] = seq + 1
-        key = (ranks, seq)
         if align > 256:
             o = _sz()
             check(lib().bg_arena_alloc_aligned(self._ctx, nbytes, int(align), ctypes.byref(o)))
             off, t = o.value, self._arena_u8[o.value: o.value + nbytes]
         else:
             off, t = self.alloc(nbytes)
-        buf = SymBuffer(self, group, nbytes, off, t, key)
+        return self._add_sym(group, nbytes, off, t, registered=False)
+
+    def sym_register(self, group, byte_offset, nbytes):
+        """A symmetric buffer over an existing range ``[byte_offset, byte_offset + nbytes)`` of this rank's arena -- memory another
+        buffer already owns, such as one parameter's slice of a unit's gradient buffer.  Same ordering rule as ``sym_alloc`` (it
+        takes the group's next sequence number); peer offsets become known at the next ``exchange()``, which also refuses a
+        registration whose size differs between the members.  Offset and size: whole 16-B vectors."""
+        byte_offset, nbytes = int(byte_offset), int(nbytes)
+        used = _sz()
+        check(lib().bg_arena_info(self._ctx, None, None, ctypes.byref(used)))
+        if byte_offset % 16 or nbytes % 16 or nbytes <= 0 or byte_offset + nbytes > used.value:
+            raise BgError("sym_register: [%d, +%d) is not a 16-B aligned range of allocated arena memory" % (byte_offset, nbytes))
+        return self._add_sym(group, nbytes, byte_offset, self._arena_u8[byte_offset: byte_offset + nbytes], registered=True)
+
+    def _add_sym(self, group, nbytes, off, t, registered):
+        ranks = tuple(group.ranks)
+        seq = self._sym_seq.get(ranks, 0)
+        self._sym_seq[ranks] = seq + 1
+        key = (ranks, seq)
+        buf = SymBuffer(self, group, nbytes, off, t, key, registered=registered)
         self._sym[key] = buf
         if group.size > 1:
             self._pending.append(buf)
         return buf
 
     def exchange(self, pg=None):
-        """Collective over the whole job: learn the peers' offsets of every pending symmetric buffer."""
-        mine = {b.key: b.offset for b in self._pending}
+        """Collective over the whole job: learn the peers' offsets of every pending symmetric buffer (and check that every member
+        registered the same number of bytes for a ``sym_register`` buffer)."""
+        mine = {b.key: (b.offset, b.nbytes) for b in self._pending}
         if self._local_peers is not None:
-            tables = {c.rank: {b.key: b.offset for b in c._sym.values()} for c in self._local_peers}
+            tables = {c.rank: {b.key: (b.offset, b.nbytes) for b in c._sym.values()} for c in self._local_peers}
         elif self.world == 1:
             tables = {self.rank: mine}
         else:
@@ -465,7 +485,12 @@ class BgComm:
             for r in b.group.ranks:
                 if b.key not in tables[r]:
                     raise BgError("rank %d did not allocate symmetric buffer %r (allocation order differs)" % (r, b.key))
-                offs.append(tables[r][b.key])
+                off, nbytes = tables[r][b.key]
+                if b.registered and nbytes != b.nbytes:
+                    raise BgError("registered symmetric buffer %r: %d bytes on rank %d, %d on rank %d -- the members' ranges must have "
+                                  "the same size (tied embeddings: the same vocabulary sharding on both rows)"
+                                  % (b.key, b.nbytes, self.rank, nbytes, r))
+                offs.append(off)
             b.offsets = (_sz * len(offs))(*offs)
         self._pending = []
 
@@ -555,6 +580,13 @@ class BgComm:
         with self._in_order(stream) as sp:
             check(lib().bg_all_reduce(self._ctx, self.group_id(group), lane, offs, _ptr(dst), n, dtype_code(dst.dtype), op,
                                       float(scale), sp))
+
+    def pair_sum_inplace(self, group, buf, dtype, elems=None, scale=1.0, lane=LANE_REDUCE, stream=None):
+        """Both members' ``buf`` (SymBuffer of a two-member ``group``, first ``elems`` elements of ``dtype``) <- scale * (x0 + x1)."""
+        import torch
+        n = buf.nbytes // torch.empty((), dtype=dtype).element_size() if elems is None else int(elems)
+        with self._in_order(stream) as sp:
+            check(lib().bg_pair_sum_inplace(self._ctx, self.group_id(group), lane, buf.offs(), n, dtype_code(dtype), float(scale), sp))
 
     def all_to_all_rows(self, group, descs, dtype, lane=LANE_ACT, stream=None):
         """descs: list of dicts with keys src(SymBuffer) [src_byte_offset] dst(tensor) batch rows row_elems src_bs src_rs

@@ -70,7 +70,7 @@ DEFAULTS = dict(
     fused_optimizer=False,               # AdamW inside the gradient reduce-scatter kernel (SURVEY 8f-3)
     recompute_activations=False,         # opt-in: GEMMs keep what their input was made from (SwiGLU / RMSNorm inputs) and redo the
                                          # elementwise pass in backward -- 352 MiB less per 8B layer at seq 8192
-    untie_embeddings_and_output_weights=True,   # megatron's flag; the tied path (C14, grad_reduce.py:98-131) is not built
+    untie_embeddings_and_output_weights=True,   # megatron's flag; False ties them (C14, grad_reduce.py:98-131; the reference's GPT default)
     zero3_pool_slots=4,                  # rotating peer-visible buffers the zero3 layers of one group gather into (0 = one per layer)
     cp_comm="allgather",                 # context parallelism's K/V exchange: "allgather" (whole-sequence K/V per layer, one gather) or
                                          # "ring" (only the local s/c rows kept; blocks travel between neighbours, c-1 hops)

@@ -396,6 +396,41 @@ class CudaBackend:
                                   dst_dtype=torch.float32)
         return buf.view(torch.float32, unit.padded).clone()
 
+    # ---- tied word embeddings across pipeline stages (C14): the two copies' gradient ranges, summed in place over peer memory ---------
+    supports_tied_embedding_exchange = True
+
+    def register_tied_grad(self, unit, param, group):
+        """``param``'s range of the unit's gradient buffer G as a symmetric buffer over ``group`` (the embedding group: the first and
+        the last stage, which hold the two copies of the tied matrix).  No memory of its own.  Before ``exchange()``, in the same
+        order on both members; ``exchange()`` refuses the pair when the two ranges differ in size."""
+        i = next(k for k, p in enumerate(unit.params) if p is param)
+        esz = unit.g_flat.element_size()
+        n = (unit.numels[i] + 7) // 8 * 8        # (the flat layout starts every parameter on a whole 8-element block)
+        return self.comm.sym_register(group, unit.G.offset + unit.offsets[i] * esz, n * esz)
+
+    def tied_grad_sum(self, unit, buf):
+        """Both copies' gradients (``buf`` from ``register_tied_grad``) <- their sum, in place, on the reduce stream after the
+        backward already queued; the unit's reduction, launched next on the same stream, reads the sum."""
+        with self._on_reduce_stream(unit):
+            self.comm.pair_sum_inplace(buf.group, buf, unit.reduce_dtype, lane=self.bg.LANE_REDUCE)
+        self._count("tied_pair_sum")
+
+    def tied_average(self, buf, x):
+        """fp32 ``x`` <- (x + the other member's x) / 2 in place (construction).  The matrix passes through the registered gradient
+        range -- unused before the first backward -- in as many pieces as it needs (two when G is bf16); the range is left zeroed."""
+        flat = x.view(-1)
+        stage = buf.u8.view(torch.float32)
+        cap = stage.numel() // 4 * 4
+        for lo in range(0, flat.numel(), cap):
+            k = min(cap, flat.numel() - lo)
+            kp = (k + 3) // 4 * 4
+            stage[:k].copy_(flat[lo:lo + k])
+            stage[k:kp].zero_()
+            self.comm.pair_sum_inplace(buf.group, buf, torch.float32, elems=kp, scale=0.5, lane=self.bg.LANE_REDUCE)
+            self._count("tied_pair_sum")
+            flat[lo:lo + k].copy_(stage[:k])
+        buf.u8.zero_()
+
     def barrier_all(self):
         torch.cuda.synchronize()
         import torch.distributed as dist

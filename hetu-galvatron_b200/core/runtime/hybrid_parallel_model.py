@@ -185,6 +185,7 @@ def construct_hybrid_parallel_model_api(model, model_config, training_args, hybr
                                 cp_groups_whole)
     finalize_pools(be)
     be.exchange()
+    hp_model.sync_tied_embeddings()     # (a collective over the peer buffers: only now are their offsets known)
 
     gm = GalvatronModel(hp_model)
     gm.dp_groups_whole, gm.tp_groups_whole, gm.sp_groups_whole = dp_groups_whole, tp_groups_whole, sp_groups_whole

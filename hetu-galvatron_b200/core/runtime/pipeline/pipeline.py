@@ -166,6 +166,7 @@ class PipelineParallel(nn.Module):
         self.async_grad_reduce = args.async_grad_reduce
         self.embedding_group, self.tied_wte_attr_names = embedding_group, tied_wte_attr_names
         self._tied_units = []           # filled by _setup_tied_embeddings once the stage's units exist
+        self._tied_grad = None          # the tied gradient range registered over the embedding group (peer-memory backend, pp > 1)
         self.units = []
         self._links = {}
         self.real_chunks = self.chunks
@@ -220,10 +221,12 @@ class PipelineParallel(nn.Module):
 
     def _setup_tied_embeddings(self):
         """``sync_embedding`` (pipeline.py:228-242): the input embedding (first unit of the first stage) and the output head (last unit
-        of the last stage) hold two copies of ONE matrix.  At construction both become the average of the two initialisations --
-        what the reference's all-reduce(AVG) over the embedding group does; after every backward their unsharded gradients are summed
-        into both (``finalize_wte_grads_func`` :1031-1050 -- the reference's pp > 1 rule, applied here for pp = 1 too, where the
-        reference averages sequentially and lets the copies drift apart), so identical optimizer steps keep them identical."""
+        of the last stage) hold two copies of ONE matrix.  At construction both become the average of the two initialisations
+        (``sync_tied_embeddings``); after every backward their unsharded gradients are summed into both (``finalize_wte_grads_func``
+        :1031-1050 -- the reference's pp > 1 rule, applied here for pp = 1 too, where the reference averages sequentially and lets the
+        copies drift apart), so identical optimizer steps keep them identical.  This step finds the tied units and parameters; across
+        pipeline stages on a peer-memory backend it also registers the parameter's gradient range over the embedding group, which the
+        in-place sum of the two copies then works on (before the backend's ``exchange()``, like every symmetric buffer)."""
         be = get_backend()
         first, last = self.is_pipeline_first_stage(), self.is_pipeline_last_stage()
         embed = self.units[0] if first else None
@@ -234,15 +237,27 @@ class PipelineParallel(nn.Module):
         if self.group_size > 1 and not getattr(be, "supports_tied_embedding_exchange", False):
             raise NotImplementedError("tied embeddings across pipeline stages need an all-reduce over the embedding group (first + last "
                                       "stage): not wired into this backend; run with untie_embeddings_and_output_weights=True or pp_deg=1")
-        fulls = []
         for u, attr in mine:
             if u.g_pool is not None:
                 raise ValueError("tied embeddings cannot use pooled zero3 gradient buffers (set --embed_sdp 0 or --zero3_pool_slots 0)")
             name, p = self._tied_param(u, attr)
             u._tie = {"param": p, "name": name, "deferred": False}
-            full = be.gather_master(u).clone()
-            fulls.append((u, full, u.named_slices(full)[name]))
             self._tied_units.append(u)
+        register = getattr(be, "register_tied_grad", None)
+        if self.group_size > 1 and register is not None:
+            u = self._tied_units[0]
+            self._tied_grad = register(u, u._tie["param"], self.embedding_group)
+
+    def sync_tied_embeddings(self):
+        """Construction, after the backend's ``exchange()``: both copies of the tied matrix become the fp32 average of the two
+        initialisations -- what the reference's all-reduce(AVG) over the embedding group does."""
+        if not self._tied_units:
+            return
+        be = get_backend()
+        fulls = []
+        for u in self._tied_units:
+            full = be.gather_master(u).clone()
+            fulls.append((u, full, u.named_slices(full)[u._tie["name"]]))
         if self.group_size == 1:
             (_, _, a), (_, _, b) = fulls
             if a.shape != b.shape:
@@ -250,6 +265,9 @@ class PipelineParallel(nn.Module):
             avg = (a + b) / 2
             a.copy_(avg)
             b.copy_(avg)
+        elif self._tied_grad is not None:
+            (_, _, a), = fulls
+            be.tied_average(self._tied_grad, a)
         else:
             (_, _, a), = fulls
             a.copy_(be.all_reduce(a.contiguous(), self.embedding_group) / 2)
@@ -273,6 +291,8 @@ class PipelineParallel(nn.Module):
                 a, b = (u._tie["param"]._bg_grad for u in self._tied_units)
                 a.add_(b)
                 b.copy_(a)
+            elif self._tied_grad is not None:
+                be.tied_grad_sum(self._tied_units[0], self._tied_grad)
             else:
                 g = self._tied_units[0]._tie["param"]._bg_grad
                 g.copy_(be.all_reduce(g.contiguous(), self.embedding_group))

@@ -524,6 +524,49 @@ __global__ void BG_SLIM all_reduce_nvls_kernel(char* mc, const char* local, char
 }
 
 // ------------------------------------------------------------------------------------------------
+// C14: in-place sum of a two-member group's copies (the tied word-embedding gradient of the first and the last pipeline stage)
+// ------------------------------------------------------------------------------------------------
+// Member m owns the vector range [lo, hi) (half of the buffer); CTA c of member m reads it from both members' regions, forms
+// scale * (x0 + x1) in fp32 -- member order fixed, one rounding, so both copies end bit-identical -- and stores it into both.  No
+// member reads a range another member writes, so one entry and one exit barrier per CTA channel are the whole protocol: both
+// members launch the same grid (it depends on the element count only), and vector v of a range is always handled by CTA c.
+template <bool kBf16>
+__global__ void BG_SLIM pair_sum_kernel(const __grid_constant__ PeerPtrs buf, size_t lo, size_t hi, float scale, const __grid_constant__ Sig s) {
+    constexpr int E = kBf16 ? 8 : 4;
+    constexpr int U = kInFlight / 2;     // two loads per vector: 8 in flight per thread
+    sync_peers<false, false, true>(s);   // both regions are complete (each member's producers precede this kernel in its stream)
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t v0 = lo + (size_t)blockIdx.x * blockDim.x + threadIdx.x; v0 < hi; v0 += stride * U) {
+        uint4 x0[U], x1[U];                // member 0's copy, member 1's copy
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const size_t v = v0 + u * stride;
+            if (v < hi) {
+                if (s.me == 0) {
+                    x0[u] = ld16_stream(buf.p[0] + v * 16);
+                    x1[u] = ld16_peer(buf.p[1] + v * 16);
+                } else {
+                    x0[u] = ld16_peer(buf.p[0] + v * 16);
+                    x1[u] = ld16_stream(buf.p[1] + v * 16);
+                }
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const size_t v = v0 + u * stride;
+            if (v >= hi) break;
+            float acc[E];
+            ar_combine<kBf16, false>(x0[u], acc, true);
+            ar_combine<kBf16, false>(x1[u], acc, false);
+            const uint4 o = ar_pack<kBf16>(acc, scale);
+            st16(buf.p[0] + v * 16, o);
+            st16(buf.p[1] + v * 16, o);
+        }
+    }
+    sync_peers<true, true, false>(s);    // my stores are visible at the peer, and the peer's have landed here
+}
+
+// ------------------------------------------------------------------------------------------------
 // C10: Ulysses all-to-all fused with the head/seq transpose (pull; up to 4 tensors per launch)
 // ------------------------------------------------------------------------------------------------
 constexpr int kMaxA2A = 4;
@@ -695,6 +738,8 @@ int bg_preload_coll() {
         K(cp_ring_release_kernel),
         K(all_reduce_nvls_kernel<true>),
         K(all_reduce_nvls_kernel<false>),
+        K(pair_sum_kernel<true>),
+        K(pair_sum_kernel<false>),
         K((all_gather_push_kernel<float, __nv_bfloat16, true>)),
         K((all_gather_push_kernel<float, __nv_bfloat16, false>)),
         K((all_gather_push_kernel<__nv_bfloat16, __nv_bfloat16, true>)),
@@ -976,6 +1021,30 @@ extern "C" int bg_all_reduce(bg_ctx_t c, int gid, int lane, const size_t* src_of
     else BG_AR_DISPATCH(all_reduce_oneshot_kernel, nvec, 1);
 #undef BG_AR_DISPATCH
 #undef BG_AR_P
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_pair_sum_inplace(bg_ctx_t c, int gid, int lane, const size_t* offs, size_t elems, int dtype, float scale, void* stream) {
+    Sig s; const Group* g;
+    int rc = make_sig(c, gid, lane, &s, &g);
+    if (rc) return rc;
+    if (g->n != 2) return fail(BG_EINVAL, "bg_pair_sum_inplace: group of %d member(s), needs exactly 2", g->n);
+    if (dtype != BG_BF16 && dtype != BG_F32) return fail(BG_EUNSUPPORTED, "bg_pair_sum_inplace dtype %d", dtype);
+    const int per = dtype == BG_BF16 ? 8 : 4;
+    if (elems % per) return fail(BG_EINVAL, "bg_pair_sum_inplace: elems %zu is not a whole number of 16-B vectors (%d elements)", elems, per);
+    PeerPtrs buf;
+    rc = resolve(c, *g, offs, elems * (dtype == BG_BF16 ? 2 : 4), &buf);
+    if (rc) return rc;
+    if (elems == 0) return BG_OK;
+    s.site = 17;
+    BG_CUDA(cudaSetDevice(c->device));
+    const size_t nvec = elems / per, half = (nvec + 1) / 2;
+    const size_t lo = g->me == 0 ? 0 : half, hi = g->me == 0 ? half : nvec;
+    const int grid = comm_grid(half / (kInFlight / 2) + 1, kThreads, g->n);     // the same on both members
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == BG_BF16) pair_sum_kernel<true><<<grid, kThreads, 0, st>>>(buf, lo, hi, scale, s);
+    else pair_sum_kernel<false><<<grid, kThreads, 0, st>>>(buf, lo, hi, scale, s);
     BG_CHECK_LAUNCH();
     return BG_OK;
 }

@@ -76,7 +76,7 @@ int bg_ctx_error_flag(bg_ctx_t ctx, int* flag);                         /* devic
  * [2] = CTA; [3] = thread or tile; [4] = value last seen; [5], [6] = group index/size or expected count/tiles;
  * [7] = launch site of a barrier timeout (1 all-gather, 2 reduce-scatter, 3 all-reduce, 6 all-to-all, 7 entry barrier of a fused
  * GEMM, 8 exit barrier of the all-reduce tile reducer, 10/11 p2p flags, 12 push kernel of the fused all-gather+GEMM, 13 cp ring
- * K/V push, 14 cp ring wait, 15 cp ring release, 16 cp ring accumulate-and-forward push), kind 4 = the
+ * K/V push, 14 cp ring wait, 15 cp ring release, 16 cp ring accumulate-and-forward push, 17 in-place pair sum), kind 4 = the
  * gathering GEMM's TMA producer waiting for a block.
  * The reference's analogue is the NCCL watchdog's timeout dump (ProcessGroupNCCL); here a lost peer traps the
  * kernel and leaves this record in mapped host memory. */
@@ -152,6 +152,14 @@ int bg_adamw_clipped(float* param, float* exp_avg, float* exp_avg_sq, const floa
  * One-shot below the "oneshot_bytes" tunable, two-shot (reduce own slice, then gather) above. */
 int bg_all_reduce(bg_ctx_t ctx, int gid, int lane, const size_t* src_offs, void* dst, size_t elems, int dtype,
                   int redop, float scale, void* stream);
+
+/* C14  tied word embeddings across pipeline stages: the first and the last stage hold two copies of one matrix, and after the
+ * backward both gradients become their sum (finalize_wte_grads_func, pipeline.py:1031-1050, an all-reduce over the embedding
+ * group).  IN PLACE over a group of exactly two members, `offs` the members' arena offsets of `elems` elements (bf16 or fp32, a
+ * whole number of 16-B vectors): on return both regions hold scale * (x0 + x1), summed in fp32 in member order and rounded once,
+ * bit-identical on both.  Member m reads and writes half of the vectors in both regions; no staging buffer, no copy.
+ * BG_EINVAL for a group of another size or a partial vector, BG_EUNSUPPORTED for another dtype; timeouts are site 17. */
+int bg_pair_sum_inplace(bg_ctx_t ctx, int gid, int lane, const size_t* offs, size_t elems, int dtype, float scale, void* stream);
 
 /* C10  Ulysses all-to-all fused with the head/seq transpose (one pass, q/k/v in one launch).
  * Replaces transformer.py:1928-1987 single_all_to_all (permute+contiguous, dist.all_to_all_single :1977,

@@ -1,5 +1,5 @@
 """Micro-benchmarks of the C-ABI kernels on one GPU (CUDA events, warm-up, L2-exceeding inputs).
-Usage: python scripts/bench_kernels.py [gemm] [cast] [ops] [attn] [dropout] [cp] [clip]  -> JSON lines on stdout.
+Usage: python scripts/bench_kernels.py [gemm] [cast] [ops] [attn] [dropout] [cp] [clip] [tied]  -> JSON lines on stdout.
        cp's head shape and sequence lengths: --cp-heads N --cp-kv-heads N --cp-head-dim N --cp-seqs S1,S2 (defaults: Llama-3.2-1B)."""
 import json
 import os
@@ -452,6 +452,72 @@ def clip():
         print(json.dumps({"bench": "clip_torch_tail_total", "unit": unit, "ms": round(total, 4)}), flush=True)
         del p, m, v, grad
         torch.cuda.empty_cache()
+
+
+def tied(vocab=50257, hidden=4096):
+    """Tied word embeddings across two pipeline stages (C14) at the GPT-3 6.7B embedding (50257 x 4096), vocab-tp 1 and 2, bf16 and
+    fp32 gradients: ``bg_pair_sum_inplace`` on the two copies' gradient ranges against what an all-reduce needs (copy into a staging
+    buffer, ``bg_all_reduce`` into a temporary, copy back), both for two virtual ranks on this one device -- so every peer access is
+    local HBM, not NVLink.  GB/s per member over the algorithmic bytes of the in-place sum: a member reads E/2 elements of its own
+    copy and E/2 of the peer's, and writes as many into each (4 x E/2 x element size); both members run at once on the device."""
+    import subprocess
+    from hetu_galvatron_b200.core.runtime.comm_groups import CommGroup
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    print(json.dumps({"nvidia_smi": q.stdout.strip()}), flush=True)
+    group = CommGroup([0, 1])
+    for t in (1, 2):
+        elems = vocab * hidden // t // 8 * 8
+        for dt in (BF, torch.float32):
+            nbytes = elems * torch.empty((), dtype=dt).element_size()
+            comms = bg.BgComm.local_world(2, device=0, arena_bytes=2 * nbytes + (16 << 20))
+            grads = [c.alloc(nbytes) for c in comms]
+            regs = [c.sym_register(group, off, nbytes) for c, (off, _) in zip(comms, grads)]
+            stage = [c.sym_alloc(group, nbytes) for c in comms]
+            for c in comms:
+                c.exchange()
+            for _, g in grads:
+                g.view(dt).copy_(torch.randn(elems, device="cuda").to(dt) * 1e-3)
+            tmp = [torch.empty(elems, dtype=dt, device="cuda") for _ in comms]
+            streams = [torch.cuda.Stream() for _ in comms]
+
+            def both(fn):
+                cur = torch.cuda.current_stream()
+                for s in streams:
+                    s.wait_stream(cur)
+                for r in range(2):
+                    with torch.cuda.stream(streams[r]):
+                        fn(r)
+                for s in streams:
+                    cur.wait_stream(s)
+
+            def pair(r):
+                comms[r].pair_sum_inplace(group, regs[r], dt, scale=0.5)
+
+            def staged(r):
+                stage[r].u8.copy_(grads[r][1])
+                comms[r].all_reduce(group, stage[r], tmp[r], scale=0.5, lane=bg.LANE_REDUCE)
+                grads[r][1].view(dt).copy_(tmp[r])
+            res = {"pair": [], "staged": []}
+            for _ in range(3):                       # interleaved rounds
+                res["pair"].append(timeit(lambda: both(pair), iters=10))
+                res["staged"].append(timeit(lambda: both(staged), iters=10))
+            torch.cuda.synchronize()
+            for c in comms:
+                assert c.error_flag() == 0
+            alg = 4 * (elems // 2) * (nbytes // elems)
+            med = {k: sorted(v)[1] for k, v in res.items()}
+            for k in ("pair", "staged"):
+                print(json.dumps({"bench": "tied_" + k, "vocab_tp": t, "dtype": str(dt).split(".")[-1], "elems": elems, "ms": round(med[k], 4),
+                                  "GBps_algorithmic_per_member": round(alg / med[k] / 1e6, 1),
+                                  "spread_pct": round(100 * (max(res[k]) - min(res[k])) / min(res[k]), 1),
+                                  "extra_arena_bytes_per_member": 0 if k == "pair" else nbytes,
+                                  "path": "local HBM (two virtual ranks on one device), not NVLink"}), flush=True)
+            print(json.dumps({"bench": "tied_staged_over_pair", "vocab_tp": t, "dtype": str(dt).split(".")[-1],
+                              "ratio": round(med["staged"] / med["pair"], 3)}), flush=True)
+            for c in comms:
+                c.close()
+            del grads, regs, stage, tmp
+            torch.cuda.empty_cache()
 
 
 if __name__ == "__main__":
