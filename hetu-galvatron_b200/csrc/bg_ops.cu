@@ -798,7 +798,8 @@ extern "C" int bg_cast(const void* src, int src_dtype, void* dst, int dst_dtype,
 }
 
 static int norm_args(long long rows, long long cols, const char* who) {
-    if (rows < 0 || cols <= 0 || cols % 8) return fail(BG_EINVAL, "%s: cols %lld must be a positive multiple of 8", who, cols);
+    if (rows < 0) return fail(BG_EINVAL, "%s: rows %lld must be >= 0", who, rows);
+    if (cols <= 0 || cols % 8) return fail(BG_EINVAL, "%s: cols %lld must be a positive multiple of 8", who, cols);
     if (cols / 8 > (long long)kMaxVpt * kThreads) return fail(BG_EUNSUPPORTED, "%s: cols %lld > %d", who, cols, kMaxVpt * kThreads * 8);
     return BG_OK;
 }
@@ -921,8 +922,10 @@ extern "C" int bg_ce_bwd(void* logits, int dtype, const long long* target, const
 
 extern "C" int bg_layernorm_fwd(const void* x, const void* w, const void* b, void* y, float* mean, float* rstd, long long rows,
                                 long long cols, float eps, void* stream) {
-    if (cols % 8 || cols > (long long)kThreads * 8 * kMaxVpt) return fail(BG_EINVAL, "layernorm: cols %lld must be a multiple of 8 and <= %d", cols, kThreads * 8 * kMaxVpt);
-    if (rows <= 0) return BG_OK;
+    int rc = norm_args(rows, cols, "bg_layernorm_fwd");
+    if (rc) return rc;
+    if (!BG_ALIGNED16(x) || !BG_ALIGNED16(w) || !BG_ALIGNED16(b) || !BG_ALIGNED16(y)) return fail(BG_EINVAL, "bg_layernorm_fwd: 16-B alignment");
+    if (rows == 0) return BG_OK;
     const int grid = (int)(rows < g_tun.local_ctas ? rows : g_tun.local_ctas);
     layernorm_fwd_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const uint4*)x, (const uint4*)w, (const uint4*)b, (uint4*)y, mean, rstd,
                                                                       rows, (int)(cols / 8), eps);
@@ -932,8 +935,12 @@ extern "C" int bg_layernorm_fwd(const void* x, const void* w, const void* b, voi
 
 extern "C" int bg_layernorm_bwd(const void* dy, const void* x, const void* w, const float* mean, const float* rstd, void* dx,
                                 float* dw_partial, float* db_partial, long long rows, long long cols, int n_partial, void* stream) {
-    if (cols % 8 || cols > (long long)kThreads * 8 * kMaxVpt) return fail(BG_EINVAL, "layernorm: cols %lld must be a multiple of 8 and <= %d", cols, kThreads * 8 * kMaxVpt);
-    if (n_partial < 1) return fail(BG_EINVAL, "layernorm_bwd: n_partial must be >= 1");
+    int rc = norm_args(rows, cols, "bg_layernorm_bwd");
+    if (rc) return rc;
+    if (n_partial < 1) return fail(BG_EINVAL, "bg_layernorm_bwd: n_partial must be >= 1");
+    if (!BG_ALIGNED16(dy) || !BG_ALIGNED16(x) || !BG_ALIGNED16(w) || !BG_ALIGNED16(dx) || !BG_ALIGNED16(dw_partial) || !BG_ALIGNED16(db_partial))
+        return fail(BG_EINVAL, "bg_layernorm_bwd: 16-B alignment");
+    // (rows == 0 still launches: every one of the n_partial CTAs writes its partial rows, zeros if it visits no row)
     layernorm_bwd_kernel<<<n_partial, kThreads, 0, (cudaStream_t)stream>>>((const uint4*)dy, (const uint4*)x, (const uint4*)w, mean, rstd, (uint4*)dx,
                                                                            dw_partial, db_partial, rows, (int)(cols / 8));
     BG_CHECK_LAUNCH();
@@ -942,7 +949,8 @@ extern "C" int bg_layernorm_bwd(const void* dy, const void* x, const void* w, co
 
 extern "C" int bg_bias_gelu(const void* x, const void* bias, const void* dy, void* out, long long rows, long long cols, int tanh_form,
                             void* stream) {
-    if (cols % 8) return fail(BG_EINVAL, "bias_gelu: cols %lld must be a multiple of 8", cols);
+    if (cols <= 0 || cols % 8) return fail(BG_EINVAL, "bg_bias_gelu: cols %lld must be a positive multiple of 8", cols);
+    if (!BG_ALIGNED16(x) || !BG_ALIGNED16(bias) || !BG_ALIGNED16(dy) || !BG_ALIGNED16(out)) return fail(BG_EINVAL, "bg_bias_gelu: 16-B alignment");
     if (rows <= 0) return BG_OK;
     const int grid = local_grid((size_t)rows * cols / 8, kThreads);
     cudaStream_t st = (cudaStream_t)stream;

@@ -65,6 +65,60 @@ def test_errors_are_return_codes(bg):
     assert bg.get_tunable("comm_ctas") == 132      # one slim CTA per SM
 
 
+# Bad-argument calls of the LayerNorm and bias-GeLU entries, each with the status and message it must return.  They run in a child
+# process that sees no device (CUDA_VISIBLE_DEVICES=""), so a call that slips past validation fails with BG_ECUDA at its launch
+# instead of launching a kernel on a bad pointer.
+_BAD_ROW_CALLS = r"""
+import json, sys
+sys.path.insert(0, sys.argv[1])
+from hetu_galvatron_b200 import _bg
+L = _bg.lib()
+A, M = 0x10000, 0x10002            # a 16-B aligned and a misaligned address; neither is ever dereferenced
+EINVAL, EUNSUPPORTED = -1, -7
+out = []
+def call(want_rc, want_msg, name, *args):
+    before = L.bg_launch_count()
+    rc = getattr(L, name)(*args)
+    out.append(dict(call="%s%r" % (name, args), got=[rc, L.bg_last_error().decode(), L.bg_launch_count() - before],
+                    want=[want_rc, want_msg, 0]))
+FWD, BWD, GELU = "bg_layernorm_fwd", "bg_layernorm_bwd", "bg_bias_gelu"
+for i in range(4):                 # x, w, b, y
+    p = [A] * 4; p[i] = M
+    call(EINVAL, FWD + ": 16-B alignment", FWD, *p, A, A, 4, 768, 1e-5, None)
+for i in (0, 1, 2, 5, 6, 7):       # dy, x, w, dx, dw_partial, db_partial (mean and rstd are read as scalars)
+    p = [A] * 8; p[i] = M
+    call(EINVAL, BWD + ": 16-B alignment", BWD, *p, 4, 768, 7, None)
+for rows, cols, rc, why in ((4, 0, EINVAL, "cols 0 must be a positive multiple of 8"),
+                            (4, -8, EINVAL, "cols -8 must be a positive multiple of 8"),
+                            (4, 12, EINVAL, "cols 12 must be a positive multiple of 8"),
+                            (-1, 768, EINVAL, "rows -1 must be >= 0"),
+                            (4, 8200, EUNSUPPORTED, "cols 8200 > 8192")):
+    call(rc, FWD + ": " + why, FWD, A, A, A, A, A, A, rows, cols, 1e-5, None)
+    call(rc, BWD + ": " + why, BWD, A, A, A, A, A, A, A, A, rows, cols, 7, None)
+call(EINVAL, BWD + ": n_partial must be >= 1", BWD, A, A, A, A, A, A, A, A, 4, 768, 0, None)
+for i in range(4):                 # x, bias, dy, out
+    p = [A] * 4; p[i] = M
+    call(EINVAL, GELU + ": 16-B alignment", GELU, *p, 4, 768, 1, None)
+call(EINVAL, GELU + ": 16-B alignment", GELU, M, None, None, A, 4, 768, 0, None)
+for cols in (0, 12):
+    call(EINVAL, GELU + ": cols %d must be a positive multiple of 8" % cols, GELU, A, None, None, A, 4, cols, 1, None)
+print(json.dumps(out))
+"""
+
+
+def test_row_ops_reject_bad_arguments(bg):
+    """LayerNorm and bias-GeLU validate their arguments as RMSNorm does, before any launch: BG_EINVAL for a negative row count,
+    a width that is not a positive multiple of 8, a pointer that is not 16-B aligned (their 16-B vector accesses would fault)
+    and no backward partials; BG_EUNSUPPORTED for a row wider than the register-resident 8192 columns."""
+    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
+    res = subprocess.run([sys.executable, "-c", _BAD_ROW_CALLS, ROOT], env=env, capture_output=True, text=True, timeout=300)
+    assert res.returncode == 0, res.stderr
+    calls = json.loads(res.stdout.strip().splitlines()[-1])
+    assert len(calls) == 4 + 6 + 10 + 1 + 5 + 2
+    bad = [c for c in calls if c["got"] != c["want"]]
+    assert not bad, bad
+
+
 def test_c_mirror_of_group_builder_matches_goldens(bg):
     L = bg.lib()
     gold = json.load(open(os.path.join(ROOT, "tests", "golden", "comm_groups.json")))
