@@ -1168,12 +1168,23 @@ extern "C" int bg_cp_ring_release(bg_ctx_t c, int gid, int kind, int parity, siz
 // ------------------------------------------------------------------------------------------------
 // fused GEMM + collective entry points (kernels in bg_gemm.cu)
 // ------------------------------------------------------------------------------------------------
-int bg_gemm_scatter_launch(const void* a, const void* b, long long m, long long n, long long k, int layout, int p, int me,
-                           void* const* partial_ptrs, uint32_t* const* flag_ptrs, void* out, void* const* bcast_ptrs, char* bcast_mc,
-                           unsigned long long timeout_ns, int* err_dev, cudaStream_t st);
-int bg_gemm_gather_launch(const void* a_local, const void* a_staged, const void* b, void* c, long long m, long long n, long long k,
-                          int layout, int p, int me, const uint32_t* flags, uint32_t target, unsigned long long timeout_ns, int* err_dev,
-                          cudaStream_t st);
+// The checks every fused GEMM entry makes before it touches the context: layout in [0, max_layout], m, n, k positive multiples
+// of 8 (TMA needs 16-B row strides), and the local operands 16-B aligned (TMA bases; the tile reducer's 16-B stores into out).
+static int fused_gemm_args(const char* who, int layout, int max_layout, long long m, long long n, long long k, const void* p0,
+                           const void* p1, const void* p2, const char* names) {
+    if (layout < 0 || layout > max_layout) return fail(BG_EINVAL, "%s: layout %d", who, layout);
+    if (m <= 0 || n <= 0 || k <= 0 || m % 8 || n % 8 || k % 8)
+        return fail(BG_EINVAL, "%s: m,n,k (%lld,%lld,%lld) must be positive multiples of 8", who, m, n, k);
+    if (((uintptr_t)p0 | (uintptr_t)p1 | (uintptr_t)p2) % 16) return fail(BG_EINVAL, "%s: %s must be 16-B aligned", who, names);
+    return BG_OK;
+}
+
+// ... and the checks that need the group: at least two members, and M split into whole 128-row blocks per member
+static int fused_gemm_group(const char* who, const Group& g, long long m) {
+    if (g.n < 2) return fail(BG_EINVAL, "%s needs a group of >= 2 ranks (use bg_gemm_bf16)", who);
+    if (m % ((long long)g.n * 128)) return fail(BG_EINVAL, "%s: M=%lld must be a multiple of p*128", who, m);
+    return BG_OK;
+}
 
 static size_t scatter_flag_count(long long m, long long n, int p) { return (size_t)((m / p + 127) / 128) * ((n + 127) / 128); }
 
@@ -1181,25 +1192,32 @@ static size_t scatter_flag_count(long long m, long long n, int p) { return (size
 extern "C" int bg_gemm_reduce_scatter(bg_ctx_t c, int gid, int lane, const void* a, const void* b, long long m, long long n,
                                       long long k, int layout, const size_t* partial_offs, const size_t* flag_offs, void* out,
                                       void* stream) {
-    Sig s; const Group* g;
-    int rc = make_sig(c, gid, lane, &s, &g);
+    static const char* who = "bg_gemm_reduce_scatter";
+    int rc = fused_gemm_args(who, layout, 2, m, n, k, a, b, out, "a, b and out");
     if (rc) return rc;
-    if (g->n < 2) return fail(BG_EINVAL, "bg_gemm_reduce_scatter needs a group of >= 2 ranks (use bg_gemm_bf16)");
+    Sig s; const Group* g;
+    rc = make_sig(c, gid, lane, &s, &g);
+    if (rc) return rc;
+    rc = fused_gemm_group(who, *g, m);
+    if (rc) return rc;
     PeerPtrs partial, flags;
     rc = resolve(c, *g, partial_offs, (size_t)m * n * 2, &partial);
     if (rc) return rc;
     rc = resolve(c, *g, flag_offs, scatter_flag_count(m, n, g->n) * sizeof(uint32_t), &flags);
     if (rc) return rc;
     BG_CUDA(cudaSetDevice(c->device));
+    void* pp[BG_MAX_PEERS]; uint32_t* fp[BG_MAX_PEERS];
+    for (int i = 0; i < BG_MAX_PEERS; ++i) { pp[i] = partial.p[i]; fp[i] = (uint32_t*)flags.p[i]; }
+    FusedGemmMaps maps;
+    rc = bg_gemm_scatter_maps(&maps, a, b, m, n, k, layout, g->n, pp);
+    if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     // Entry barrier: every member's previous use of the partial buffers and counters (its last reducer, earlier in this same
     // stream) has drained before any peer may store into them again.
     s.site = 7;
     coll_barrier_kernel<<<1, 32, 0, st>>>(s);
     BG_CHECK_LAUNCH();
-    void* pp[BG_MAX_PEERS]; uint32_t* fp[BG_MAX_PEERS];
-    for (int i = 0; i < BG_MAX_PEERS; ++i) { pp[i] = partial.p[i]; fp[i] = (uint32_t*)flags.p[i]; }
-    return bg_gemm_scatter_launch(a, b, m, n, k, layout, g->n, g->me, pp, fp, out, nullptr, nullptr,
+    return bg_gemm_scatter_launch(maps, m, n, k, layout, g->n, g->me, pp, fp, out, nullptr, nullptr,
                                   (unsigned long long)g_tun.timeout_ms * 1000000ull, c->err_dev, st);
 }
 
@@ -1209,10 +1227,14 @@ extern "C" int bg_gemm_reduce_scatter(bg_ctx_t c, int gid, int lane, const void*
 // the reducers leave through a cross-rank barrier, so `out` is complete on every member in stream order.
 extern "C" int bg_gemm_all_reduce(bg_ctx_t c, int gid, int lane, const void* a, const void* b, long long m, long long n, long long k,
                                   int layout, const size_t* partial_offs, const size_t* flag_offs, const size_t* out_offs, void* stream) {
-    Sig s; const Group* g;
-    int rc = make_sig(c, gid, lane, &s, &g);
+    static const char* who = "bg_gemm_all_reduce";
+    int rc = fused_gemm_args(who, layout, 2, m, n, k, a, b, nullptr, "a and b");
     if (rc) return rc;
-    if (g->n < 2) return fail(BG_EINVAL, "bg_gemm_all_reduce needs a group of >= 2 ranks (use bg_gemm_bf16)");
+    Sig s; const Group* g;
+    rc = make_sig(c, gid, lane, &s, &g);
+    if (rc) return rc;
+    rc = fused_gemm_group(who, *g, m);
+    if (rc) return rc;
     PeerPtrs partial, flags, outs;
     rc = resolve(c, *g, partial_offs, (size_t)m * n * 2, &partial);
     if (rc) return rc;
@@ -1221,15 +1243,18 @@ extern "C" int bg_gemm_all_reduce(bg_ctx_t c, int gid, int lane, const void* a, 
     rc = resolve(c, *g, out_offs, (size_t)m * n * 2, &outs);
     if (rc) return rc;
     BG_CUDA(cudaSetDevice(c->device));
+    void* pp[BG_MAX_PEERS]; uint32_t* fp[BG_MAX_PEERS]; void* op[BG_MAX_PEERS];
+    for (int i = 0; i < BG_MAX_PEERS; ++i) { pp[i] = partial.p[i]; fp[i] = (uint32_t*)flags.p[i]; op[i] = outs.p[i]; }
+    FusedGemmMaps maps;
+    rc = bg_gemm_scatter_maps(&maps, a, b, m, n, k, layout, g->n, pp);
+    if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     s.site = 7;
     coll_barrier_kernel<<<1, 32, 0, st>>>(s);     // previous users of partial / out / counters have drained on every member
     BG_CHECK_LAUNCH();
     s.site = 8;                                   // the reducers' exit barrier
-    void* pp[BG_MAX_PEERS]; uint32_t* fp[BG_MAX_PEERS]; void* op[BG_MAX_PEERS];
-    for (int i = 0; i < BG_MAX_PEERS; ++i) { pp[i] = partial.p[i]; fp[i] = (uint32_t*)flags.p[i]; op[i] = outs.p[i]; }
     char* mc = g_tun.nvls_bcast ? mc_ptr(c, gid, *g, out_offs, (size_t)m * n * 2) : nullptr;
-    rc = bg_gemm_scatter_launch(a, b, m, n, k, layout, g->n, g->me, pp, fp, outs.p[g->me], op, mc,
+    rc = bg_gemm_scatter_launch(maps, m, n, k, layout, g->n, g->me, pp, fp, outs.p[g->me], op, mc,
                                 (unsigned long long)g_tun.timeout_ms * 1000000ull, c->err_dev, st);
     if (rc) return rc;
     // Exit barrier, behind the reducer in the stream: my rows are in every member's result (the reducer grid has completed, its
@@ -1246,13 +1271,15 @@ extern "C" int bg_gemm_all_reduce(bg_ctx_t c, int gid, int lane, const void* a, 
 extern "C" int bg_all_gather_gemm(bg_ctx_t c, int gid, int lane, const void* a_local, const size_t* stage_offs, const size_t* flag_offs,
                                   const void* b, void* out, long long m, long long n, long long k, int layout, void* stream,
                                   void* comm_stream) {
+    static const char* who = "bg_all_gather_gemm";
+    int rc = fused_gemm_args(who, layout, 1, m, n, k, a_local, b, out, "a_local, b and c");
+    if (rc) return rc;
     Sig s; const Group* g;
-    int rc = make_sig(c, gid, lane, &s, &g);
+    rc = make_sig(c, gid, lane, &s, &g);
+    if (rc) return rc;
+    rc = fused_gemm_group(who, *g, m);
     if (rc) return rc;
     const int p = g->n;
-    if (p < 2) return fail(BG_EINVAL, "bg_all_gather_gemm needs a group of >= 2 ranks (use bg_gemm_bf16)");
-    if (layout != 0 && layout != 1) return fail(BG_EINVAL, "bg_all_gather_gemm: layout 0 (TN) or 1 (NN); the gathered operand is A[M,K]");
-    if (m % ((long long)p * 128) || k % 8 || n % 8) return fail(BG_EINVAL, "bg_all_gather_gemm: M=%lld must be a multiple of p*128, K and N of 8", m);
     const long long rows_local = m / p;
     const int n_chunks = (int)(rows_local / 128);
     PeerPtrs stage, flags;
@@ -1261,6 +1288,9 @@ extern "C" int bg_all_gather_gemm(bg_ctx_t c, int gid, int lane, const void* a_l
     rc = resolve(c, *g, flag_offs, (size_t)p * n_chunks * sizeof(uint32_t), &flags);
     if (rc) return rc;
     BG_CUDA(cudaSetDevice(c->device));
+    FusedGemmMaps maps;
+    rc = bg_gemm_gather_maps(&maps, a_local, stage.p[g->me], b, out, m, n, k, layout, p);
+    if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream, cs = (cudaStream_t)comm_stream;
     cudaEvent_t ev_in, ev_out;
     {
@@ -1292,7 +1322,7 @@ extern "C" int bg_all_gather_gemm(bg_ctx_t c, int gid, int lane, const void* a_l
         BG_CHECK_LAUNCH();
     }
     BG_CUDA(cudaEventRecord(ev_out, cs));
-    rc = bg_gemm_gather_launch(a_local, stage.p[g->me], b, out, m, n, k, layout, p, g->me, (const uint32_t*)flags.p[g->me], (uint32_t)sg.split,
+    rc = bg_gemm_gather_launch(maps, m, n, k, layout, p, g->me, (const uint32_t*)flags.p[g->me], (uint32_t)sg.split,
                                (unsigned long long)g_tun.timeout_ms * 1000000ull, c->err_dev, st);
     if (rc) return rc;
     BG_CUDA(cudaMemsetAsync(flags.p[g->me], 0, (size_t)p * n_chunks * sizeof(uint32_t), st));   // peers count again only after the next entry barrier

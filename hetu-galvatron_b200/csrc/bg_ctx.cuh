@@ -121,3 +121,20 @@ int comm_grid(size_t work_items, int threads, int n);
 // multicast (NVLS) address of a symmetric buffer: non-null when the group has a bound multicast region that covers
 // [offs[i], offs[i]+bytes) and every member placed the buffer at the same arena offset
 char* mc_ptr(bg_ctx* c, int gid, const Group& g, const size_t* offs, size_t bytes);
+
+// Fused GEMM + collective kernels (bg_gemm.cu).  The tensor maps are encoded by *_maps before the entry point (bg_coll.cu)
+// launches anything -- its entry barrier or push kernel -- so an operand the encoder rejects fails the call with no work queued
+// and no peer left waiting.  *_launch then only launches.
+struct FusedGemmMaps {
+    CUtensorMap a, b, c;               // reduce-scatter: c unused; all-gather: a = the staging buffer [M][K]
+    CUtensorMap peer[BG_MAX_PEERS];    // reduce-scatter: owner i's partial buffer; all-gather: peer[0] = the local shard
+};
+int bg_gemm_scatter_maps(FusedGemmMaps* maps, const void* a, const void* b, long long m, long long n, long long k, int layout, int p,
+                         void* const* partial_ptrs);
+int bg_gemm_scatter_launch(const FusedGemmMaps& maps, long long m, long long n, long long k, int layout, int p, int me,
+                           void* const* partial_ptrs, uint32_t* const* flag_ptrs, void* out, void* const* bcast_ptrs, char* bcast_mc,
+                           unsigned long long timeout_ns, int* err_dev, cudaStream_t st);
+int bg_gemm_gather_maps(FusedGemmMaps* maps, const void* a_local, const void* a_staged, const void* b, void* c, long long m, long long n,
+                        long long k, int layout, int p);
+int bg_gemm_gather_launch(const FusedGemmMaps& maps, long long m, long long n, long long k, int layout, int p, int me,
+                          const uint32_t* flags, uint32_t target, unsigned long long timeout_ns, int* err_dev, cudaStream_t st);

@@ -710,36 +710,39 @@ __global__ void __launch_bounds__(128, 8) tile_reduce_kernel(const __nv_bfloat16
 
 }  // namespace
 
-// Internal entry used by bg_coll.cu (which owns contexts, groups and peer pointers).  partial/flags: per-member pointers.
-// Both kernels go to ONE stream: the GEMM, then the reducer as its programmatic dependent (it starts when all GEMM CTAs are
-// resident, not when they finish; tiles are handed over through the arrival counters).
-int bg_gemm_scatter_launch(const void* a, const void* b, long long m, long long n, long long k, int layout, int p, int me,
+// Internal entries used by bg_coll.cu (which owns contexts, groups and peer pointers and has validated the arguments: layout,
+// dims, alignment, p >= 2, M % (p * 128)).  partial/flags: per-member pointers.  Both kernels go to ONE stream: the GEMM, then
+// the reducer as its programmatic dependent (it starts when all GEMM CTAs are resident, not when they finish; tiles are handed
+// over through the arrival counters).
+int bg_gemm_scatter_maps(FusedGemmMaps* maps, const void* a, const void* b, long long m, long long n, long long k, int layout, int p,
+                         void* const* partial_ptrs) {
+    int rc = make_ab_maps(&maps->a, &maps->b, a, b, m, n, k, layout);
+    if (rc) return rc;
+    for (int i = 0; i < BG_MAX_PEERS; ++i) {
+        if (i < p) { rc = make_map(&maps->peer[i], partial_ptrs[i], m, n, kStoreCols, BLOCK_M); if (rc) return rc; }
+        else maps->peer[i] = maps->peer[0];
+    }
+    return gemm_setup();
+}
+
+int bg_gemm_scatter_launch(const FusedGemmMaps& maps, long long m, long long n, long long k, int layout, int p, int me,
                            void* const* partial_ptrs, uint32_t* const* flag_ptrs, void* out, void* const* bcast_ptrs, char* bcast_mc,
                            unsigned long long timeout_ns, int* err_dev, cudaStream_t st) {
-    if (layout < 0 || layout > 2) return fail(BG_EINVAL, "bg_gemm_reduce_scatter: layout %d", layout);
-    if (m <= 0 || n <= 0 || k <= 0 || n % 8 || k % 8) return fail(BG_EINVAL, "bg_gemm_reduce_scatter: bad dims");
-    if (m % ((long long)p * BLOCK_M)) return fail(BG_EINVAL, "bg_gemm_reduce_scatter: M=%lld must be a multiple of p*%d", m, BLOCK_M);
     const int rows_per_rank = (int)(m / p);
-    CUtensorMap ma, mb;
-    int rc = make_ab_maps(&ma, &mb, a, b, m, n, k, layout);
-    if (rc) return rc;
     FuseParams<kScatterMode> sp;
     sp.p = p; sp.me = me; sp.rows_per_rank = rows_per_rank;
     for (int i = 0; i < BG_MAX_PEERS; ++i) {
         sp.flags[i] = i < p ? flag_ptrs[i] : nullptr;
-        if (i < p) { rc = make_map(&sp.dst[i], partial_ptrs[i], (long long)p * rows_per_rank, n, kStoreCols, BLOCK_M); if (rc) return rc; }
-        else sp.dst[i] = sp.dst[0];
+        sp.dst[i] = maps.peer[i];
     }
-    rc = gemm_setup();
-    if (rc) return rc;
     const int m_blocks = (int)((m + BLOCK_M - 1) / BLOCK_M), n_blocks = (int)((n + BLOCK_N - 1) / BLOCK_N);
     const long long tiles = (long long)m_blocks * n_blocks;
     const int grid = (int)(tiles < g_num_sms ? tiles : g_num_sms);
     const int local_tiles = (rows_per_rank / BLOCK_M) * n_blocks;
     const CUtensorMap& mc_unused = sp.dst[0];
-    if (layout == kTN) gemm_bf16_kernel<kTN, kScatterMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(ma, mb, mc_unused, nullptr, (int)m, (int)n, (int)k, 0, sp);
-    else if (layout == kNN) gemm_bf16_kernel<kNN, kScatterMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(ma, mb, mc_unused, nullptr, (int)m, (int)n, (int)k, 0, sp);
-    else gemm_bf16_kernel<kNT, kScatterMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(ma, mb, mc_unused, nullptr, (int)m, (int)n, (int)k, 0, sp);
+    if (layout == kTN) gemm_bf16_kernel<kTN, kScatterMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(maps.a, maps.b, mc_unused, nullptr, (int)m, (int)n, (int)k, 0, sp);
+    else if (layout == kNN) gemm_bf16_kernel<kNN, kScatterMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(maps.a, maps.b, mc_unused, nullptr, (int)m, (int)n, (int)k, 0, sp);
+    else gemm_bf16_kernel<kNT, kScatterMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(maps.a, maps.b, mc_unused, nullptr, (int)m, (int)n, (int)k, 0, sp);
     BG_CHECK_LAUNCH();
     // one reducer CTA fits beside a GEMM CTA (registers); more CTAs than SMs only queue
     const int rgrid = local_tiles < g_num_sms ? local_tiles : g_num_sms;
@@ -763,27 +766,27 @@ int bg_gemm_scatter_launch(const void* a, const void* b, long long m, long long 
 }
 
 // Fused all-gather + GEMM: the consumer half (the push kernel is launched by bg_coll.cu on the communication stream).
-int bg_gemm_gather_launch(const void* a_local, const void* a_staged, const void* b, void* c, long long m, long long n, long long k,
-                          int layout, int p, int me, const uint32_t* flags, uint32_t target, unsigned long long timeout_ns, int* err_dev,
-                          cudaStream_t st) {
-    if (layout != kTN && layout != kNN) return fail(BG_EINVAL, "bg_all_gather_gemm: layout %d", layout);
-    if (((uintptr_t)a_local | (uintptr_t)a_staged | (uintptr_t)b | (uintptr_t)c) % 16) return fail(BG_EINVAL, "bg_all_gather_gemm: pointers must be 16-B aligned");
-    CUtensorMap ma, mb, mc;
-    int rc = make_ab_maps(&ma, &mb, a_staged, b, m, n, k, layout);
+int bg_gemm_gather_maps(FusedGemmMaps* maps, const void* a_local, const void* a_staged, const void* b, void* c, long long m, long long n,
+                        long long k, int layout, int p) {
+    int rc = make_ab_maps(&maps->a, &maps->b, a_staged, b, m, n, k, layout);
     if (rc) return rc;
-    rc = make_map(&mc, c, m, n, kStoreCols, BLOCK_M);
+    rc = make_map(&maps->c, c, m, n, kStoreCols, BLOCK_M);
     if (rc) return rc;
+    rc = make_map(&maps->peer[0], a_local, m / p, k, BLOCK_K, BLOCK_M);
+    if (rc) return rc;
+    return gemm_setup();
+}
+
+int bg_gemm_gather_launch(const FusedGemmMaps& maps, long long m, long long n, long long k, int layout, int p, int me,
+                          const uint32_t* flags, uint32_t target, unsigned long long timeout_ns, int* err_dev, cudaStream_t st) {
     FuseParams<kGatherMode> gp;
-    rc = make_map(&gp.a_local, a_local, m / p, k, BLOCK_K, BLOCK_M);
-    if (rc) return rc;
+    gp.a_local = maps.peer[0];
     gp.flags = flags; gp.target = target; gp.p = p; gp.me = me; gp.blocks_per_rank = (int)(m / p / BLOCK_M);
     gp.timeout_ns = timeout_ns; gp.err = err_dev;
-    rc = gemm_setup();
-    if (rc) return rc;
     const long long tiles = (m / BLOCK_M) * ((n + BLOCK_N - 1) / BLOCK_N);
     const int grid = (int)(tiles < g_num_sms ? tiles : g_num_sms);
-    if (layout == kTN) gemm_bf16_kernel<kTN, kGatherMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(ma, mb, mc, nullptr, (int)m, (int)n, (int)k, 0, gp);
-    else gemm_bf16_kernel<kNN, kGatherMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(ma, mb, mc, nullptr, (int)m, (int)n, (int)k, 0, gp);
+    if (layout == kTN) gemm_bf16_kernel<kTN, kGatherMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(maps.a, maps.b, maps.c, nullptr, (int)m, (int)n, (int)k, 0, gp);
+    else gemm_bf16_kernel<kNN, kGatherMode><<<grid, kThreads, Tile<BLOCK_N>::kSmemBytes, st>>>(maps.a, maps.b, maps.c, nullptr, (int)m, (int)n, (int)k, 0, gp);
     BG_CHECK_LAUNCH();
     return BG_OK;
 }

@@ -286,8 +286,12 @@ int bg_gemm_bf16_add(const void* a, const void* b, void* c, const void* addend, 
  * counted there; a tile reducer on the owner -- launched into the same stream as the GEMM's programmatic dependent, so it
  * runs beside the GEMM CTAs once all of them are resident -- sums the p partials as they land and writes out[M/p, N].
  * Replaces layers.py:1061-1109 (row-parallel GEMM then mappings_group.py:120 reduce-scatter) and :462,488-494 (dgrad +
- * reduce-scatter).  partial_offs: symmetric bf16 buffer of M*N elements; flag_offs: symmetric u32[(M/p/128)*ceil(N/256)],
- * zero-initialised.  M must be a multiple of p*128.  `out` is complete in stream order. */
+ * reduce-scatter).  partial_offs: symmetric bf16 buffer of M*N elements; flag_offs: symmetric u32[(M/p/128)*ceil(N/128)],
+ * zero-initialised.  `out` is complete in stream order.
+ * Returns BG_EINVAL, in this order, for: layout outside 0-2; m, n or k not a positive multiple of 8; a, b or out not 16-B
+ * aligned; a null ctx or a bad lane (bad gid: BG_EGROUP); a group of fewer than 2 members; M not a multiple of p*128; a symmetric
+ * offset that is not 16-B aligned or a buffer outside the arena.  A failed call -- these, or a tensor-map encode that rejects an
+ * operand (BG_ECUDA) -- has launched nothing, on this member or for its peers. */
 int bg_gemm_reduce_scatter(bg_ctx_t ctx, int gid, int lane, const void* a, const void* b, long long m, long long n, long long k,
                            int layout, const size_t* partial_offs, const size_t* flag_offs, void* out, void* stream);
 
@@ -296,7 +300,8 @@ int bg_gemm_reduce_scatter(bg_ctx_t ctx, int gid, int lane, const void* a, const
  * operation: partial tiles are scattered to their owners as in bg_gemm_reduce_scatter; the owner's tile reducer sums a tile when
  * its p partials have landed and immediately broadcasts the rows into EVERY member's out buffer (peer stores, or one multimem.st
  * when out is multicast-bound); the reducers leave through a cross-rank barrier, so out -- a symmetric bf16 [M][N] buffer,
- * out_offs -- is complete on every member in stream order.  Deterministic (fixed summation order), fp32 accumulation. */
+ * out_offs -- is complete on every member in stream order.  Deterministic (fixed summation order), fp32 accumulation.
+ * BG_EINVAL as bg_gemm_reduce_scatter (with no `out` pointer to check: out is symmetric); a failed call has launched nothing. */
 int bg_gemm_all_reduce(bg_ctx_t ctx, int gid, int lane, const void* a, const void* b, long long m, long long n, long long k, int layout,
                        const size_t* partial_offs, const size_t* flag_offs, const size_t* out_offs, void* stream);
 
@@ -306,7 +311,11 @@ int bg_gemm_all_reduce(bg_ctx_t ctx, int gid, int lane, const void* a, const voi
  * every member's staging buffer (stage_offs: symmetric bf16 [M][K]) in 128-row blocks and counts each block in on the receiver
  * (flag_offs: symmetric u32[p][M/p/128], zero-initialised); the GEMM's TMA producer reads the rank's own rows from a_local and
  * every remote block from staging as soon as its counter is complete, walking the blocks in arrival order.  layout 0 (TN) or
- * 1 (NN); M a multiple of p*128.  C is complete in `stream` order; a_local may be reused after the call in `stream` order. */
+ * 1 (NN).  C is complete in `stream` order; a_local may be reused after the call in `stream` order.
+ * Returns BG_EINVAL, in this order, for: layout outside 0-1; m, n or k not a positive multiple of 8; a_local, b or c not 16-B
+ * aligned; a null ctx or a bad lane (bad gid: BG_EGROUP); a group of fewer than 2 members; M not a multiple of p*128; a symmetric
+ * offset that is not 16-B aligned or a buffer outside the arena.  A failed call -- these, or a tensor-map encode that rejects an
+ * operand (BG_ECUDA) -- has launched nothing: no push, no GEMM, no wait on either stream. */
 int bg_all_gather_gemm(bg_ctx_t ctx, int gid, int lane, const void* a_local, const size_t* stage_offs, const size_t* flag_offs,
                        const void* b, void* c, long long m, long long n, long long k, int layout, void* stream, void* comm_stream);
 

@@ -119,6 +119,71 @@ def test_row_ops_reject_bad_arguments(bg):
     assert not bad, bad
 
 
+# Bad-argument calls of the plain GEMM entries, and the context-free bad arguments of the fused GEMM + collective entries (called
+# with a null context: every check that needs no context comes first).  Same child process as above, with no device.
+_BAD_GEMM_CALLS = r"""
+import json, sys
+sys.path.insert(0, sys.argv[1])
+from hetu_galvatron_b200 import _bg
+L = _bg.lib()
+A, M = 0x10000, 0x10008            # a 16-B aligned and an 8-B aligned address; neither is ever dereferenced
+EINVAL = -1
+out = []
+def call(want_msg, name, *args):
+    before = L.bg_launch_count()
+    rc = getattr(L, name)(*args)
+    out.append(dict(call="%s%r" % (name, args), got=[rc, L.bg_last_error().decode(), L.bg_launch_count() - before],
+                    want=[EINVAL, want_msg, 0]))
+GEMM, ADD = "bg_gemm_bf16", "bg_gemm_bf16_add"
+BAD_DIMS = ((0, 64, 64), (64, 0, 64), (64, 64, 0), (-8, 64, 64), (64, -8, 64), (64, 64, -8), (12, 64, 64), (64, 12, 64),
+            (64, 64, 12))
+for layout in (-1, 3):
+    call(GEMM + ": layout %d" % layout, GEMM, A, A, A, 64, 64, 64, layout, 0, None)
+    call(GEMM + ": layout %d" % layout, ADD, A, A, A, A, 64, 64, 64, layout, None)
+for m, n, k in BAD_DIMS:
+    why = GEMM + ": m,n,k (%d,%d,%d) must be positive multiples of 8" % (m, n, k)
+    call(why, GEMM, A, A, A, m, n, k, 0, 1, None)
+    call(why, ADD, A, A, A, A, m, n, k, 1, None)
+for i in range(3):                 # a, b, c
+    p = [A] * 3; p[i] = M
+    call(GEMM + ": pointers must be 16-B aligned", GEMM, *p, 64, 64, 64, 2, 0, None)
+    call(GEMM + ": pointers must be 16-B aligned", ADD, *p, A, 64, 64, 64, 2, None)
+for addend in (None, M):
+    call(ADD + ": addend must be a 16-B aligned [M][N] bf16 tensor", ADD, A, A, A, addend, 64, 64, 64, 0, None)
+RS, AR, AG = "bg_gemm_reduce_scatter", "bg_gemm_all_reduce", "bg_all_gather_gemm"
+def rs(layout=0, m=256, n=64, k=64, a=A, b=A, o=A):
+    return (None, 0, 2, a, b, m, n, k, layout, None, None, o, None)
+def ar(layout=0, m=256, n=64, k=64, a=A, b=A):
+    return (None, 0, 2, a, b, m, n, k, layout, None, None, None, None)
+def ag(layout=0, m=256, n=64, k=64, a=A, b=A, c=A):
+    return (None, 0, 4, a, None, None, b, c, m, n, k, layout, None, None)
+for name, make, layouts, ptrs in ((RS, rs, (-1, 3), ("a", "b", "o")), (AR, ar, (-1, 3), ("a", "b")), (AG, ag, (-1, 2), ("a", "b", "c"))):
+    names = {RS: "a, b and out", AR: "a and b", AG: "a_local, b and c"}[name]
+    for layout in layouts:
+        call(name + ": layout %d" % layout, name, *make(layout=layout))
+    for m, n, k in BAD_DIMS:
+        call(name + ": m,n,k (%d,%d,%d) must be positive multiples of 8" % (m, n, k), name, *make(m=m, n=n, k=k))
+    for ptr in ptrs:
+        call(name + ": %s must be 16-B aligned" % names, name, *make(**{ptr: M}))
+    call("null ctx", name, *make())             # every context-free argument valid: the context is checked next
+print(json.dumps(out))
+"""
+
+
+def test_gemm_entries_reject_bad_arguments(bg):
+    """The plain GEMM entries, and the fused GEMM + reduce-scatter / all-reduce / all-gather entries, reject a bad layout, a
+    dimension that is not a positive multiple of 8 and an operand that is not 16-B aligned (TMA bases and strides; the tile
+    reducer's 16-B stores into `out`) with BG_EINVAL before any launch.  The fused entries make these checks before they look
+    at the context, so a call that fails them can never have launched an entry barrier or a push that its peers then wait on."""
+    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
+    res = subprocess.run([sys.executable, "-c", _BAD_GEMM_CALLS, ROOT], env=env, capture_output=True, text=True, timeout=300)
+    assert res.returncode == 0, res.stderr
+    calls = json.loads(res.stdout.strip().splitlines()[-1])
+    assert len(calls) == 2 * (2 + 9 + 3) + 2 + (2 + 9 + 3 + 1) + (2 + 9 + 2 + 1) + (2 + 9 + 3 + 1)
+    bad = [c for c in calls if c["got"] != c["want"]]
+    assert not bad, bad
+
+
 def test_c_mirror_of_group_builder_matches_goldens(bg):
     L = bg.lib()
     gold = json.load(open(os.path.join(ROOT, "tests", "golden", "comm_groups.json")))

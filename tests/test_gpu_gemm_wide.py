@@ -11,6 +11,8 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from _fp_check import assert_rounded, gemm_eps  # noqa: E402
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 BF = torch.bfloat16
 
@@ -48,7 +50,8 @@ def test_wide_tile_matches_narrow_slices(bg, layout, m, n, k, epilogue):
         part = gemm(bs, c0[:, c_lo:c_hi].contiguous(), c_hi - c_lo)
         torch.cuda.synchronize()
         assert torch.equal(part, full[:, c_lo:c_hi]), (c_lo, c_hi)
-    want = (a.float().t() if layout == 2 else a.float()) @ (b.float().t() if layout == 0 else b.float())
-    want += c0.float() if epilogue else 0
-    err = (full.float() - want).abs()
-    assert (err <= want.abs() * 2 ** -7 + 1e-3 * (k ** 0.5)).all(), float(err.max())
+    ad, bd = (a.double().t() if layout == 2 else a.double()), (b.double().t() if layout == 0 else b.double())
+    ref, s = ad @ bd, ad.abs() @ bd.abs()
+    if epilogue:
+        ref, s = ref + c0.double(), s + c0.double().abs()
+    assert_rounded(full, ref, gemm_eps(k, s))       # the fp32 accumulation bound, then one correct bf16 rounding

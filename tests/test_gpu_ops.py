@@ -23,10 +23,9 @@ import torch
 import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from _fp_check import BF, F64, U, _bits, assert_rounded, assert_within, gamma, ulp_f32  # noqa: E402
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(600)]
-BF = torch.bfloat16
-F64 = torch.float64
-U = 2.0 ** -24              # unit roundoff of fp32
 NAN = float("nan")
 
 
@@ -51,60 +50,9 @@ def _nan(*shape, dtype=torch.float32):
     return torch.full(shape, NAN, device="cuda", dtype=dtype)
 
 
-def gamma(k):
-    """Higham's gamma_k = k u / (1 - k u): the relative error bound of k fp32 roundings in a row."""
-    return k * U / (1 - k * U)
-
-
 def _f32_rel(c):
     """relative difference between the fp32 literal a kernel uses and the exact constant c"""
     return abs(float(np.float32(c)) - c) / abs(c)
-
-
-def _ulp(v, mant):
-    """spacing of the floating-point numbers with `mant` explicit mantissa bits at |v|: 2^(floor(log2|v|) - mant)
-    (normal range; the smallest normal's spacing below it)"""
-    _, e = torch.frexp(v.double().abs().clamp_min(2.0 ** -126))
-    return torch.ldexp(torch.ones_like(v, dtype=F64), e - 1 - mant)
-
-
-def ulp_bf16(v):
-    return _ulp(v, 7)
-
-
-def ulp_f32(v):
-    return _ulp(v, 23)
-
-
-def _report(what, got, ref, err, tol, bad):
-    i = int(torch.argmax(torch.where(bad, (err / tol).nan_to_num(float("inf")), torch.zeros_like(err))))
-    flat = lambda t: t.reshape(-1)[i].item()  # noqa: E731
-    return (f"{what}: {int(bad.sum())} / {bad.numel()} outside the bound; worst at flat index {i}: got {flat(got)} ref {flat(ref)} "
-            f"err {flat(err):.3e} tol {flat(tol):.3e}")
-
-
-def assert_rounded(got, ref, eps, what="bf16 output"):
-    """bf16 `got` against the float64 `ref`: |got - ref| <= 1/2 ulp_bf16 + eps, the ulp the larger of got's and ref's (a result
-    rounded up across a power of two is still correctly rounded).  NaN anywhere fails."""
-    assert got.dtype == BF and ref.dtype == F64
-    g = got.double()
-    tol = 0.5 * torch.maximum(ulp_bf16(g), ulp_bf16(ref)) + eps
-    err = (g - ref).abs()
-    bad = ~(err <= tol)
-    assert not bad.any(), _report(what, g, ref, err, tol, bad)
-
-
-def assert_within(got, ref, eps, what="fp32 output"):
-    """fp32 `got` against the float64 `ref`: |got - ref| <= eps + 1/2 ulp_fp32 (the final rounding of the fp32 result)."""
-    g = got.double()
-    tol = eps + 0.5 * ulp_f32(ref)
-    err = (g - ref).abs()
-    bad = ~(err <= tol)
-    assert not bad.any(), _report(what, g, ref, err, tol, bad)
-
-
-def _bits(t):
-    return t.view(torch.int16) if t.dtype == BF else t.view(torch.int32)
 
 
 def _tree_depth(cols, threads=256, per_vec=8):
