@@ -818,22 +818,40 @@ int bg_preload_coll() {
 // =================================================================================================================
 // entry points
 // =================================================================================================================
+// Every plain collective entry below makes its context-free checks (dtypes, whole 16-B vectors, local pointer alignment,
+// descriptor fields) before make_sig, then the group and arena checks; a call that fails any of them has launched nothing.
+
+// bytes = count * unit of a symmetric buffer, refused as resolve() refuses a buffer outside the arena when the product exceeds the
+// arena -- checked before it is formed, so an absurd count cannot wrap it to a small size that resolve() would accept
+static int sym_bytes(const bg_ctx* c, size_t count, size_t unit, size_t* bytes) {
+    if (unit != 0 && count > c->arena_bytes / unit)
+        return fail(BG_EINVAL, "symmetric buffer of %zu x %zu B outside arena", count, unit);
+    *bytes = count * unit;
+    return BG_OK;
+}
+
 static int launch_all_gather(bg_ctx_t c, int gid, int lane, const void* src, int src_dtype, const size_t* dst_offs, int dst_dtype,
                              size_t shard_elems, const AgSignal* sg, void* stream) {
-    Sig s; const Group* g;
-    int rc = make_sig(c, gid, lane, &s, &g);
-    if (rc) return rc;
+    if (!(src_dtype == BG_F32 && dst_dtype == BG_BF16) && !(src_dtype == BG_BF16 && dst_dtype == BG_BF16) &&
+        !(src_dtype == BG_F32 && dst_dtype == BG_F32))
+        return fail(BG_EUNSUPPORTED, "all_gather_cast %d->%d", src_dtype, dst_dtype);
     const size_t dsz = dst_dtype == BG_BF16 ? 2 : 4;
     const int per = (src_dtype == BG_F32 && dst_dtype == BG_F32) ? 4 : 8;
     if (shard_elems % per) return fail(BG_EINVAL, "shard_elems %zu must be a multiple of %d (pad the flat buffer)", shard_elems, per);
     if ((uintptr_t)src % 16) return fail(BG_EINVAL, "src not 16-B aligned");
+    Sig s; const Group* g;
+    int rc = make_sig(c, gid, lane, &s, &g);
+    if (rc) return rc;
+    size_t bytes;
+    rc = sym_bytes(c, shard_elems, (size_t)g->n * dsz, &bytes);
+    if (rc) return rc;
     PeerPtrs dst;
-    rc = resolve(c, *g, dst_offs, shard_elems * g->n * dsz, &dst);
+    rc = resolve(c, *g, dst_offs, bytes, &dst);
     if (rc) return rc;
     if (shard_elems == 0) return BG_OK;
     s.site = sg ? 12 : 1;
     BG_CUDA(cudaSetDevice(c->device));
-    char* mc = (sg == nullptr && g_tun.nvls_gather) ? mc_ptr(c, gid, *g, dst_offs, shard_elems * g->n * dsz) : nullptr;
+    char* mc = (sg == nullptr && g_tun.nvls_gather) ? mc_ptr(c, gid, *g, dst_offs, bytes) : nullptr;
     if (mc && shard_elems * dsz < (size_t)g_tun.nvls_min_bytes) mc = nullptr;
     int grid = comm_grid(shard_elems / per / kUnroll + 1, kThreads, g->n);
     cudaStream_t st = (cudaStream_t)stream;
@@ -845,8 +863,7 @@ static int launch_all_gather(bg_ctx_t c, int gid, int lane, const void* src, int
     } while (0)
     if (src_dtype == BG_F32 && dst_dtype == BG_BF16) BG_AG(float, __nv_bfloat16);
     else if (src_dtype == BG_BF16 && dst_dtype == BG_BF16) BG_AG(__nv_bfloat16, __nv_bfloat16);
-    else if (src_dtype == BG_F32 && dst_dtype == BG_F32) BG_AG(float, float);
-    else return fail(BG_EUNSUPPORTED, "all_gather_cast %d->%d", src_dtype, dst_dtype);
+    else BG_AG(float, float);
 #undef BG_AG
     BG_CHECK_LAUNCH();
     return BG_OK;
@@ -859,20 +876,24 @@ extern "C" int bg_all_gather_cast(bg_ctx_t c, int gid, int lane, const void* src
 
 static int launch_reduce_scatter(bg_ctx_t c, int gid, int lane, const size_t* src_offs, int src_dtype, int epi, RsOut o,
                                  size_t shard_elems, float prescale, float postscale, void* stream) {
-    Sig s; const Group* g;
-    int rc = make_sig(c, gid, lane, &s, &g);
-    if (rc) return rc;
+    if (src_dtype != BG_BF16 && src_dtype != BG_F32) return fail(BG_EUNSUPPORTED, "reduce_scatter src dtype %d", src_dtype);
     const int per = src_dtype == BG_BF16 ? 8 : 4;
     const size_t ssz = src_dtype == BG_BF16 ? 2 : 4;
     if (shard_elems % per) return fail(BG_EINVAL, "shard_elems %zu must be a multiple of %d", shard_elems, per);
     if ((uintptr_t)o.dst % 16) return fail(BG_EINVAL, "dst not 16-B aligned");
+    Sig s; const Group* g;
+    int rc = make_sig(c, gid, lane, &s, &g);
+    if (rc) return rc;
+    size_t bytes;
+    rc = sym_bytes(c, shard_elems, (size_t)g->n * ssz, &bytes);
+    if (rc) return rc;
     PeerPtrs src;
-    rc = resolve(c, *g, src_offs, shard_elems * g->n * ssz, &src);
+    rc = resolve(c, *g, src_offs, bytes, &src);
     if (rc) return rc;
     if (shard_elems == 0) return BG_OK;
     s.site = 2;
     BG_CUDA(cudaSetDevice(c->device));
-    const char* mc = g_tun.nvls_reduce ? mc_ptr(c, gid, *g, src_offs, shard_elems * g->n * ssz) : nullptr;
+    const char* mc = g_tun.nvls_reduce ? mc_ptr(c, gid, *g, src_offs, bytes) : nullptr;
     if (mc && shard_elems * ssz < (size_t)g_tun.nvls_min_bytes) mc = nullptr;
     const bool half = epi == kEpiAdamW || epi == kEpiAdamWClip || epi == kEpiSumSq;
     const int pmax = g->n <= 2 ? 2 : g->n <= 4 ? 4 : 8;
@@ -973,17 +994,20 @@ extern "C" int bg_adamw_clipped(float* param, float* exp_avg, float* exp_avg_sq,
 
 extern "C" int bg_all_reduce(bg_ctx_t c, int gid, int lane, const size_t* src_offs, void* dst, size_t elems, int dtype,
                              int redop, float scale, void* stream) {
-    Sig s; const Group* g;
-    int rc = make_sig(c, gid, lane, &s, &g);
-    if (rc) return rc;
     if (dtype != BG_BF16 && dtype != BG_F32) return fail(BG_EUNSUPPORTED, "all_reduce dtype %d", dtype);
     if (redop != BG_SUM && redop != BG_MAX) return fail(BG_EUNSUPPORTED, "all_reduce op %d", redop);
     const int per = dtype == BG_BF16 ? 8 : 4;
     const size_t esz = dtype == BG_BF16 ? 2 : 4;
     if (elems % per) return fail(BG_EINVAL, "all_reduce elems %zu must be a multiple of %d (pad)", elems, per);
     if ((uintptr_t)dst % 16) return fail(BG_EINVAL, "dst not 16-B aligned");
+    Sig s; const Group* g;
+    int rc = make_sig(c, gid, lane, &s, &g);
+    if (rc) return rc;
+    size_t bytes;
+    rc = sym_bytes(c, elems, esz, &bytes);
+    if (rc) return rc;
     PeerPtrs src;
-    rc = resolve(c, *g, src_offs, elems * esz, &src);
+    rc = resolve(c, *g, src_offs, bytes, &src);
     if (rc) return rc;
     if (elems == 0) return BG_OK;
     s.site = 3;
@@ -991,8 +1015,8 @@ extern "C" int bg_all_reduce(bg_ctx_t c, int gid, int lane, const size_t* src_of
     cudaStream_t st = (cudaStream_t)stream;
     const size_t nvec = elems / per;
     // large sums on a multicast-bound buffer are reduced and replicated inside the switch
-    if (redop == BG_SUM && g->n > 1 && elems * esz >= (size_t)g_tun.nvls_min_bytes) {
-        char* mc = mc_ptr(c, gid, *g, src_offs, elems * esz);
+    if (redop == BG_SUM && g->n > 1 && bytes >= (size_t)g_tun.nvls_min_bytes) {
+        char* mc = mc_ptr(c, gid, *g, src_offs, bytes);
         if (mc != nullptr) {
             const int grid = comm_grid((nvec + g->n - 1) / g->n / kInFlight + 1, kThreads, g->n);
             if (dtype == BG_BF16) all_reduce_nvls_kernel<true><<<grid, kThreads, 0, st>>>(mc, src.p[g->me], (char*)dst, nvec, scale, s);
@@ -1001,7 +1025,7 @@ extern "C" int bg_all_reduce(bg_ctx_t c, int gid, int lane, const size_t* src_of
             return BG_OK;
         }
     }
-    const bool twoshot = g->n > 1 && elems * esz > (size_t)g_tun.oneshot_bytes && nvec % g->n == 0;
+    const bool twoshot = g->n > 1 && bytes > (size_t)g_tun.oneshot_bytes && nvec % g->n == 0;
     const bool bf = dtype == BG_BF16, mx = redop == BG_MAX;
 #define BG_AR_P(KERNEL, P, NV)                                                                            \
     do {                                                                                                  \
@@ -1026,15 +1050,18 @@ extern "C" int bg_all_reduce(bg_ctx_t c, int gid, int lane, const size_t* src_of
 }
 
 extern "C" int bg_pair_sum_inplace(bg_ctx_t c, int gid, int lane, const size_t* offs, size_t elems, int dtype, float scale, void* stream) {
+    if (dtype != BG_BF16 && dtype != BG_F32) return fail(BG_EUNSUPPORTED, "bg_pair_sum_inplace dtype %d", dtype);
+    const int per = dtype == BG_BF16 ? 8 : 4;
+    if (elems % per) return fail(BG_EINVAL, "bg_pair_sum_inplace: elems %zu is not a whole number of 16-B vectors (%d elements)", elems, per);
     Sig s; const Group* g;
     int rc = make_sig(c, gid, lane, &s, &g);
     if (rc) return rc;
     if (g->n != 2) return fail(BG_EINVAL, "bg_pair_sum_inplace: group of %d member(s), needs exactly 2", g->n);
-    if (dtype != BG_BF16 && dtype != BG_F32) return fail(BG_EUNSUPPORTED, "bg_pair_sum_inplace dtype %d", dtype);
-    const int per = dtype == BG_BF16 ? 8 : 4;
-    if (elems % per) return fail(BG_EINVAL, "bg_pair_sum_inplace: elems %zu is not a whole number of 16-B vectors (%d elements)", elems, per);
+    size_t bytes;
+    rc = sym_bytes(c, elems, dtype == BG_BF16 ? 2 : 4, &bytes);
+    if (rc) return rc;
     PeerPtrs buf;
-    rc = resolve(c, *g, offs, elems * (dtype == BG_BF16 ? 2 : 4), &buf);
+    rc = resolve(c, *g, offs, bytes, &buf);
     if (rc) return rc;
     if (elems == 0) return BG_OK;
     s.site = 17;
@@ -1051,30 +1078,44 @@ extern "C" int bg_pair_sum_inplace(bg_ctx_t c, int gid, int lane, const size_t* 
 
 extern "C" int bg_all_to_all_rows(bg_ctx_t c, int gid, int lane, const bg_a2a_desc* descs, int n_descs, int dtype,
                                   void* stream) {
+    if (!descs || n_descs < 1 || n_descs > kMaxA2A) return fail(BG_EINVAL, "1..%d tensors per all_to_all launch", kMaxA2A);
+    if (dtype != BG_BF16 && dtype != BG_F32) return fail(BG_EUNSUPPORTED, "all_to_all dtype %d", dtype);
+    const long long esz = dtype == BG_BF16 ? 2 : 4, per = 16 / esz;
+    for (int i = 0; i < n_descs; ++i) {
+        const bg_a2a_desc& d = descs[i];
+        if (d.batch < 0 || d.rows < 0 || d.row_elems < 0 || d.src_bs < 0 || d.src_rs < 0 || d.src_me_off < 0 || d.dst_bs < 0 ||
+            d.dst_rs < 0 || d.dst_peer_off < 0)
+            return fail(BG_EINVAL, "all_to_all: negative extent or stride");
+        if (d.row_elems % per || d.src_bs % per || d.src_rs % per || d.src_me_off % per || d.dst_bs % per ||
+            d.dst_rs % per || d.dst_peer_off % per)
+            return fail(BG_EINVAL, "all_to_all: strides/row length must be multiples of %lld elements", per);
+        if ((uintptr_t)d.dst % 16) return fail(BG_EINVAL, "all_to_all dst not 16-B aligned");
+        // the kernel indexes a tensor's vectors of one peer with 32-bit counters
+        const unsigned long long lim = 1ull << 32, b = d.batch, r = d.rows, v = d.row_elems / per;
+        if (b && r && v && (b >= lim || r >= lim || v >= lim || b * r >= lim || b * r * v >= lim))
+            return fail(BG_EINVAL, "all_to_all: more than 2^32 16-B vectors per peer");
+    }
     Sig s; const Group* g;
     int rc = make_sig(c, gid, lane, &s, &g);
     if (rc) return rc;
-    if (!descs || n_descs < 1 || n_descs > kMaxA2A) return fail(BG_EINVAL, "1..%d tensors per all_to_all launch", kMaxA2A);
-    const long long esz = dtype == BG_BF16 ? 2 : 4, per = 16 / esz;
     A2AArgs a;
     a.n_tensors = n_descs;
     size_t max_vec = 0;
     for (int i = 0; i < n_descs; ++i) {
         const bg_a2a_desc& d = descs[i];
-        if (d.row_elems % per || d.src_bs % per || d.src_rs % per || d.src_me_off % per || d.dst_bs % per ||
-            d.dst_rs % per || d.dst_peer_off % per)
-            return fail(BG_EINVAL, "all_to_all: strides/row length must be multiples of %lld elements", per);
-        if ((uintptr_t)d.dst % 16) return fail(BG_EINVAL, "all_to_all dst not 16-B aligned");
-        // extent of the peer's source that may be touched
-        long long span = (d.batch - 1) * d.src_bs + (d.rows - 1) * d.src_rs + (long long)(g->n - 1) * d.src_me_off + d.row_elems;
-        rc = resolve(c, *g, d.src_offs, (size_t)span * esz, &a.t[i].src);
+        // extent of the peer's source that may be touched (none for an empty tensor); 128-bit, so huge strides cannot wrap it
+        // under the arena size
+        const bool empty = d.batch == 0 || d.rows == 0 || d.row_elems == 0;
+        const unsigned __int128 span = empty ? 0 : (unsigned __int128)(d.batch - 1) * d.src_bs + (unsigned __int128)(d.rows - 1) * d.src_rs +
+                                                       (unsigned __int128)(g->n - 1) * d.src_me_off + d.row_elems;
+        const unsigned __int128 bytes = span * esz;
+        rc = resolve(c, *g, d.src_offs, bytes > (unsigned __int128)SIZE_MAX ? SIZE_MAX : (size_t)bytes, &a.t[i].src);
         if (rc) return rc;
         a.t[i].dst = (char*)d.dst;
         a.t[i].batch = d.batch; a.t[i].rows = d.rows; a.t[i].row_vec = d.row_elems / per;
         a.t[i].src_bs = d.src_bs / per; a.t[i].src_rs = d.src_rs / per; a.t[i].src_me_off = d.src_me_off / per;
         a.t[i].dst_bs = d.dst_bs / per; a.t[i].dst_rs = d.dst_rs / per; a.t[i].dst_peer_off = d.dst_peer_off / per;
         a.t[i].total_vec = d.batch * d.rows * a.t[i].row_vec * g->n;
-        if (d.batch * d.rows * a.t[i].row_vec >= (1ll << 32)) return fail(BG_EINVAL, "all_to_all: more than 2^32 16-B vectors per peer");
         if ((size_t)(a.t[i].total_vec / g->n) > max_vec) max_vec = (size_t)(a.t[i].total_vec / g->n);
     }
     s.site = 6;

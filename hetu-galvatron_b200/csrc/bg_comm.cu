@@ -508,7 +508,8 @@ int resolve(bg_ctx* c, const Group& g, const size_t* offs, size_t bytes, PeerPtr
         char* base = c->peer_base[g.ranks[i]];
         if (!base) return fail(BG_ENOTMAPPED, "arena of rank %d is not mapped", g.ranks[i]);
         if (offs[i] % 16) return fail(BG_EINVAL, "symmetric offset %zu not 16-B aligned", offs[i]);
-        if (offs[i] < c->pad_bytes || offs[i] + bytes > c->arena_bytes)
+        // (written so that no sum can wrap around: a huge `bytes` must not pass as a small one)
+        if (offs[i] < c->pad_bytes || bytes > c->arena_bytes || offs[i] > c->arena_bytes - bytes)
             return fail(BG_EINVAL, "symmetric buffer [%zu,+%zu) outside arena", offs[i], bytes);
         out->p[i] = base + offs[i];
     }

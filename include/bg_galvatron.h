@@ -102,7 +102,16 @@ int bg_barrier(bg_ctx_t ctx, int gid, int lane, void* stream);
  * Replaces torch/distributed/fsdp/_flat_param.py:1477 all_gather_into_tensor (+ the MixedPrecision shard cast,
  * galvatron/core/runtime/parallel.py:116-122); also the plain activation all-gathers mappings_group.py:100,
  * layers.py:410-412, redistribute.py:65,110 when src_dtype == dst_dtype.
- * Push: every member casts its shard once and stores it into slot `my_index` of every member's dst. */
+ * Push: every member casts its shard once and stores it into slot `my_index` of every member's dst.
+ *
+ * Errors of the plain collectives (this entry, bg_reduce_scatter_acc, bg_all_reduce, bg_pair_sum_inplace, bg_all_to_all_rows),
+ * in this order: first the checks that need no context (dtypes, whole 16-B vectors, local pointer alignment, descriptor fields),
+ * then a null ctx or a bad lane (BG_EINVAL; a bad gid is BG_EGROUP), then the group's checks, then the symmetric offsets (BG_EINVAL
+ * for one that is not 16-B aligned or a buffer that does not lie inside the arena -- compared without overflow, so an element
+ * count too large for the arena is refused however large it is).  A call that fails has launched nothing, on this member or for
+ * its peers.
+ * Here: BG_EUNSUPPORTED for a dtype pair other than fp32->bf16, bf16->bf16 and fp32->fp32 (also when shard_elems is 0);
+ * BG_EINVAL for shard_elems not a multiple of 8 (of 4 for fp32->fp32) and for src not 16-B aligned. */
 int bg_all_gather_cast(bg_ctx_t ctx, int gid, int lane, const void* src, int src_dtype, const size_t* dst_offs,
                        int dst_dtype, size_t shard_elems, void* stream);
 
@@ -110,7 +119,12 @@ int bg_all_gather_cast(bg_ctx_t ctx, int gid, int lane, const void* src, int src
  * Replaces torch/distributed/fsdp/_runtime_utils.py:852 (prediv) :858 reduce_scatter_tensor :879 (postdiv)
  * :917-924 (cast to param dtype, += _saved_grad_shard), reached from sp_grad_reduce.py:125-126; with
  * dst_dtype bf16 and accumulate 0 it is the Megatron-SP reduce-scatter (mappings_group.py:120, layers.py:488-494).
- * Pull: member i reads slice i of every member's src, sums in fp32, dst = [dst +] sum * prescale * postscale. */
+ * Pull: member i reads slice i of every member's src, sums in fp32, dst = [dst +] sum * prescale * postscale.  In fp32, in this
+ * order: acc = fmaf(x_m, prescale, acc) over the members m (own slice first, then the peers in ring order), acc * postscale, then
+ * + the old dst when accumulating, then one rounding to dst's dtype.
+ * BG_EUNSUPPORTED for a dst dtype other than bf16 / fp32, a bf16 dst with an fp32 src, or a src dtype other than bf16 / fp32;
+ * BG_EINVAL for shard_elems not a multiple of 8 (bf16 src) or 4 (fp32 src) and for dst not 16-B aligned (order and the later
+ * checks: see bg_all_gather_cast). */
 int bg_reduce_scatter_acc(bg_ctx_t ctx, int gid, int lane, const size_t* src_offs, int src_dtype, void* dst,
                           int dst_dtype, size_t shard_elems, float prescale, float postscale, int accumulate,
                           void* stream);
@@ -146,10 +160,16 @@ int bg_reduce_scatter_adamw_clipped(bg_ctx_t ctx, int gid, int lane, const size_
 int bg_adamw_clipped(float* param, float* exp_avg, float* exp_avg_sq, const float* grad, size_t n, float lr, float beta1,
                      float beta2, float eps, float weight_decay, long long step, const float* clip_coef, void* stream);
 
-/* C3/C5/C6/C13/C14/C16  all-reduce (sum|max), out of place: src is a symmetric buffer, dst any local pointer.
+/* C3/C5/C6/C13/C14/C16  all-reduce (sum|max): src is a symmetric buffer, dst any local pointer.
  * Replaces _runtime_utils.py:940 (DDP grads), mappings_group.py:19 _reduce (row-parallel fwd, layers.py:1114;
  * column-parallel bwd, mappings_group.py:139), cross_entropy.py:22-30,61-72,78-89, grad_reduce.py:121-124.
- * One-shot below the "oneshot_bytes" tunable, two-shot (reduce own slice, then gather) above. */
+ * dst = scale * (sum | max over the members' src), in fp32 in member order, rounded once; every member's dst is bit-identical.
+ * One-shot up to the "oneshot_bytes" tunable, and above it whenever the vectors do not split evenly over the members; two-shot
+ * (reduce own slice, then gather) otherwise.  src is NOT left as it was in every case: the two-shot kernel writes the reduced,
+ * scaled slice `my_index` back into slice `my_index` of the member's own src (its peers gather it from there), and on a
+ * multicast-bound src (NVLS) every member's src ends up holding the whole result.  The one-shot kernel leaves src unchanged.
+ * BG_EUNSUPPORTED for a dtype other than bf16 / fp32 or an op other than BG_SUM / BG_MAX; BG_EINVAL for elems not a multiple of
+ * 8 (bf16) or 4 (fp32) and for dst not 16-B aligned (order and the later checks: see bg_all_gather_cast). */
 int bg_all_reduce(bg_ctx_t ctx, int gid, int lane, const size_t* src_offs, void* dst, size_t elems, int dtype,
                   int redop, float scale, void* stream);
 
@@ -158,13 +178,18 @@ int bg_all_reduce(bg_ctx_t ctx, int gid, int lane, const size_t* src_offs, void*
  * group).  IN PLACE over a group of exactly two members, `offs` the members' arena offsets of `elems` elements (bf16 or fp32, a
  * whole number of 16-B vectors): on return both regions hold scale * (x0 + x1), summed in fp32 in member order and rounded once,
  * bit-identical on both.  Member m reads and writes half of the vectors in both regions; no staging buffer, no copy.
- * BG_EINVAL for a group of another size or a partial vector, BG_EUNSUPPORTED for another dtype; timeouts are site 17. */
+ * BG_EUNSUPPORTED for another dtype and BG_EINVAL for a partial vector (both before the context is looked at), BG_EINVAL for a
+ * group of another size; a failed call has launched nothing.  Timeouts are site 17. */
 int bg_pair_sum_inplace(bg_ctx_t ctx, int gid, int lane, const size_t* offs, size_t elems, int dtype, float scale, void* stream);
 
 /* C10  Ulysses all-to-all fused with the head/seq transpose (one pass, q/k/v in one launch).
  * Replaces transformer.py:1928-1987 single_all_to_all (permute+contiguous, dist.all_to_all_single :1977,
  * post_all2all :1904-1925).  Pull: for each peer q and tensor t, rows of `row_elems[t]` contiguous elements:
- *   dst_t[b*dst_bs + r*dst_rs + q*dst_peer_off + c] = src_t(peer q)[b*src_bs + r*src_rs + me*src_me_off + c] */
+ *   dst_t[b*dst_bs + r*dst_rs + q*dst_peer_off + c] = src_t(peer q)[b*src_bs + r*src_rs + me*src_me_off + c]
+ * BG_EINVAL for descs null or n_descs outside 1..4; BG_EUNSUPPORTED for a dtype other than bf16 / fp32; BG_EINVAL for a negative
+ * batch, rows, row_elems or stride, a row length or stride that is not a whole number of 16-B vectors, dst not 16-B aligned, and
+ * more than 2^32 vectors of one tensor per peer.  Then as bg_all_gather_cast; the source extent checked against the arena is
+ * (batch-1)*src_bs + (rows-1)*src_rs + (n-1)*src_me_off + row_elems elements (none for an empty tensor). */
 typedef struct bg_a2a_desc {
     const size_t* src_offs; /* symmetric source (arena offsets, group order) */
     void* dst;              /* local destination */

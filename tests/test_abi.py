@@ -184,6 +184,105 @@ def test_gemm_entries_reject_bad_arguments(bg):
     assert not bad, bad
 
 
+# Bad-argument calls of the plain collective entries, with a null context: each must fail on its own context-free check, which comes
+# before the context is looked at.  The last call of each entry has every such argument valid and fails on the null context.  Same
+# child process as above, with no device.
+_BAD_COLL_CALLS = r"""
+import ctypes, json, sys
+sys.path.insert(0, sys.argv[1])
+from hetu_galvatron_b200 import _bg
+L = _bg.lib()
+A, M = 0x10000, 0x10008            # a 16-B aligned and an 8-B aligned address; neither is ever dereferenced
+EINVAL, EUNSUPPORTED = -1, -7
+BF, F32 = 0, 1
+out = []
+def call(want_rc, want_msg, name, *args):
+    before = L.bg_launch_count()
+    rc = getattr(L, name)(*args)
+    out.append(dict(call="%s%r" % (name, args), got=[rc, L.bg_last_error().decode(), L.bg_launch_count() - before],
+                    want=[want_rc, want_msg, 0]))
+AG, RS, AR, PS, A2A = "bg_all_gather_cast", "bg_reduce_scatter_acc", "bg_all_reduce", "bg_pair_sum_inplace", "bg_all_to_all_rows"
+def ag(src=A, sd=F32, dd=BF, n=64):
+    return (None, 0, 0, src, sd, None, dd, n, None)
+for sd, dd in ((BF, F32), (2, BF), (F32, 2), (-1, -1)):
+    call(EUNSUPPORTED, "all_gather_cast %d->%d" % (sd, dd), AG, *ag(sd=sd, dd=dd))
+    call(EUNSUPPORTED, "all_gather_cast %d->%d" % (sd, dd), AG, *ag(sd=sd, dd=dd, n=0))    # checked before the empty return
+for sd, dd, n, per in ((F32, BF, 4, 8), (BF, BF, 12, 8), (F32, F32, 6, 4)):
+    call(EINVAL, "shard_elems %d must be a multiple of %d (pad the flat buffer)" % (n, per), AG, *ag(sd=sd, dd=dd, n=n))
+call(EINVAL, "src not 16-B aligned", AG, *ag(src=M))
+call(EINVAL, "null ctx", AG, *ag())
+def rs(sd=BF, dst=A, dd=F32, n=64, acc=0):
+    return (None, 0, 1, None, sd, dst, dd, n, 0.5, 0.25, acc, None)
+for dd in (2, -1):
+    call(EUNSUPPORTED, "reduce_scatter dst dtype %d" % dd, RS, *rs(dd=dd))
+call(EUNSUPPORTED, "reduce_scatter 1->0", RS, *rs(sd=F32, dd=BF))
+for sd in (2, -1):
+    call(EUNSUPPORTED, "reduce_scatter src dtype %d" % sd, RS, *rs(sd=sd))
+for sd, dd, n, per in ((BF, F32, 4, 8), (BF, BF, 12, 8), (F32, F32, 6, 4)):
+    call(EINVAL, "shard_elems %d must be a multiple of %d" % (n, per), RS, *rs(sd=sd, dd=dd, n=n))
+for dd in (F32, BF):
+    call(EINVAL, "dst not 16-B aligned", RS, *rs(dd=dd, dst=M, acc=1))
+call(EINVAL, "null ctx", RS, *rs())
+def ar(dst=A, n=64, dt=BF, op=0):
+    return (None, 0, 2, None, dst, n, dt, op, 1.0 / 3.0, None)
+for dt in (2, -1):
+    call(EUNSUPPORTED, "all_reduce dtype %d" % dt, AR, *ar(dt=dt))
+for op in (2, -1):
+    call(EUNSUPPORTED, "all_reduce op %d" % op, AR, *ar(op=op))
+for dt, n, per in ((BF, 4, 8), (F32, 6, 4)):
+    call(EINVAL, "all_reduce elems %d must be a multiple of %d (pad)" % (n, per), AR, *ar(dt=dt, n=n))
+call(EINVAL, "dst not 16-B aligned", AR, *ar(dst=M))
+call(EINVAL, "null ctx", AR, *ar())
+def ps(n=64, dt=BF):
+    return (None, 0, 1, None, n, dt, 0.5, None)
+call(EUNSUPPORTED, "bg_pair_sum_inplace dtype 2", PS, *ps(dt=2))
+for dt, n, per in ((BF, 12, 8), (F32, 6, 4)):
+    call(EINVAL, "bg_pair_sum_inplace: elems %d is not a whole number of 16-B vectors (%d elements)" % (n, per), PS, *ps(n=n, dt=dt))
+call(EINVAL, "null ctx", PS, *ps())
+GOOD = dict(batch=2, rows=4, row_elems=64, src_bs=512, src_rs=128, src_me_off=64, dst_bs=512, dst_rs=64, dst_peer_off=256)
+def a2a(dt=BF, count=None, **kw):
+    ds = (_bg.bg_a2a_desc * 2)()
+    for d in ds:
+        d.dst = A
+        for k, v in dict(GOOD, **kw).items():
+            setattr(d, k, v)
+    return (None, 0, 2, ds, 2 if count is None else count, dt, None)
+call(EINVAL, "1..4 tensors per all_to_all launch", A2A, None, 0, 2, None, 1, BF, None)
+for count in (0, 5):
+    call(EINVAL, "1..4 tensors per all_to_all launch", A2A, *a2a(count=count))
+for dt in (2, -1):
+    call(EUNSUPPORTED, "all_to_all dtype %d" % dt, A2A, *a2a(dt=dt))
+for k in GOOD:
+    call(EINVAL, "all_to_all: negative extent or stride", A2A, *a2a(**{k: -GOOD[k]}))
+for k in GOOD:
+    if k not in ("batch", "rows"):
+        call(EINVAL, "all_to_all: strides/row length must be multiples of 8 elements", A2A, *a2a(**{k: GOOD[k] + 4}))
+call(EINVAL, "all_to_all: strides/row length must be multiples of 4 elements", A2A, *a2a(dt=F32, row_elems=66))
+call(EINVAL, "all_to_all dst not 16-B aligned", A2A, *a2a(dst=M))
+for b, r, e in ((1 << 16, 1 << 16, 8), (1, 1 << 20, 1 << 15), (1 << 32, 1, 8), (1 << 40, 1 << 40, 8)):
+    call(EINVAL, "all_to_all: more than 2^32 16-B vectors per peer", A2A, *a2a(batch=b, rows=r, row_elems=e))
+call(EINVAL, "null ctx", A2A, *a2a(batch=0))      # an empty tensor is valid
+call(EINVAL, "null ctx", A2A, *a2a(dt=F32))
+call(EINVAL, "null ctx", A2A, *a2a())
+print(json.dumps(out))
+"""
+
+
+def test_collectives_reject_bad_arguments(bg):
+    """The all-gather, reduce-scatter, all-reduce, pair-sum and all-to-all entries reject an unsupported dtype or dtype pair
+    (BG_EUNSUPPORTED), and an element count that is not a whole number of 16-B vectors, a misaligned local pointer, a negative
+    all-to-all extent or stride and an all-to-all of more than 2^32 vectors per peer (BG_EINVAL), with zero launches and before they
+    look at the context: a call that fails them can never have left its peers waiting."""
+    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
+    res = subprocess.run([sys.executable, "-c", _BAD_COLL_CALLS, ROOT], env=env, capture_output=True, text=True, timeout=300)
+    assert res.returncode == 0, res.stderr
+    calls = json.loads(res.stdout.strip().splitlines()[-1])
+    assert len(calls) == (8 + 3 + 1 + 1) + (2 + 1 + 2 + 3 + 2 + 1) + (2 + 2 + 2 + 1 + 1) + (1 + 2 + 1) + \
+        (1 + 2 + 2 + 9 + 7 + 1 + 1 + 4 + 3)
+    bad = [c for c in calls if c["got"] != c["want"]]
+    assert not bad, bad
+
+
 def test_c_mirror_of_group_builder_matches_goldens(bg):
     L = bg.lib()
     gold = json.load(open(os.path.join(ROOT, "tests", "golden", "comm_groups.json")))
