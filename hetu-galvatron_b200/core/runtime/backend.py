@@ -730,6 +730,48 @@ class CudaBackend:
                                                  1 if tanh_form else 0, _s()))
         return dx.view_as(x)
 
+    def bias_tanh_fwd(self, x, bias):
+        x2 = x.reshape(-1, x.shape[-1])
+        y = torch.empty_like(x2)
+        self.bg.check(self.bg.lib().bg_bias_tanh(_p(x2), _p(bias) if bias is not None else None, None, _p(y), x2.shape[0], x2.shape[1], _s()))
+        return y.view_as(x)
+
+    def bias_tanh_bwd(self, dy, x, bias):
+        x2, dy2 = x.reshape(-1, x.shape[-1]), dy.reshape(-1, x.shape[-1])
+        dx = torch.empty_like(x2)
+        self.bg.check(self.bg.lib().bg_bias_tanh(_p(x2), _p(bias) if bias is not None else None, _p(dy2), _p(dx), x2.shape[0], x2.shape[1],
+                                                 _s()))
+        return dx.view_as(x)
+
+    def vit_patchify(self, pixels, patch, rows_pad):
+        """pixels [B, C, H, W] (fp32 / bf16) -> bf16 patch rows [rows_pad, p*p*C] in (p1 p2 c) order, rows past B*P zero."""
+        b, c, hgt, wid = pixels.shape
+        pixels = pixels.contiguous()
+        out = torch.empty(rows_pad, patch * patch * c, dtype=torch.bfloat16, device=pixels.device)
+        self.bg.check(self.bg.lib().bg_vit_patchify(_p(pixels), self.bg.dtype_code(pixels.dtype), _p(out), b, c, hgt, wid, patch, rows_pad,
+                                                    _s()))
+        return out
+
+    def vit_embed_fwd(self, patch_out, bias, cls, pos, batch, s_run, p, seed, iteration, site, sample_base):
+        """-> y [s_run, batch, h]: cls + pos[0], then patch_out rows + bias + pos[1..P], then zero rows (dropout fused when p > 0)."""
+        n_patches, h = pos.shape[0] - 1, pos.shape[1]
+        y = torch.empty(s_run, batch, h, dtype=torch.bfloat16, device=patch_out.device)
+        self.bg.check(self.bg.lib().bg_vit_embed_fwd(_p(patch_out), _p(bias), _p(cls), _p(pos), _p(y), batch, n_patches, s_run, h,
+                                                     int(sample_base), float(p), int(seed), int(iteration), int(site), _s()))
+        return y
+
+    def vit_embed_bwd(self, dy, n_patches, rows_pad, p, seed, iteration, site, sample_base):
+        """-> (dpatch [rows_pad, h] bf16, dcls [h] fp32, dpos [P + 1, h] fp32, dbias [h] fp32) from dy [s_run, batch, h]."""
+        s_run, batch, h = dy.shape
+        dy = dy.contiguous()
+        dpatch = torch.empty(rows_pad, h, dtype=torch.bfloat16, device=dy.device)
+        dpos = torch.empty(n_patches + 1, h, dtype=torch.float32, device=dy.device)
+        npart = min(self.norm_partials, n_patches)
+        dbp = torch.empty(npart, h, dtype=torch.float32, device=dy.device)
+        self.bg.check(self.bg.lib().bg_vit_embed_bwd(_p(dy), _p(dpatch), _p(dpos), _p(dbp), npart, batch, n_patches, s_run, rows_pad, h,
+                                                     int(sample_base), float(p), int(seed), int(iteration), int(site), _s()))
+        return dpatch, dpos[0], dpos, dbp.sum(0)
+
     def dropout_add_fwd(self, x, bias, residual, p, seed, iteration, site, seq_base, sample_base):
         """y = residual + keep * scale * (x + bias) on an SBH tensor x [s_loc, b_loc, h] whose rows are tokens seq_base.. of samples
         sample_base.. (mask: include/bg_galvatron.h).  bias [h] (bf16 / fp32) and residual (x's shape) may be None."""

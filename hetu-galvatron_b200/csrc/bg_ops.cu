@@ -760,6 +760,161 @@ __global__ void __launch_bounds__(kThreads) lse_merge_kernel(const uint4* __rest
     if (final_out) st16(final_out + idx, pack8(f));
 }
 
+// ---------------------------------------------------------------------------------------------
+// ViT front end (vit_hf/ViTModel_sequential.py ViTEmbeddings_): patchify relayout, then the SBH activation assembled from the
+// patch GEMM's output, the patch bias, the CLS token and the learned position table, with the embedding dropout fused in.
+// ---------------------------------------------------------------------------------------------
+// pixels [B, C, H, W] -> patch rows [rows_pad, p*p*C] in einops' "b c (h p1) (w p2) -> b (h w) (p1 p2 c)" order, bf16 (one RNE
+// rounding for fp32 pixels); rows B*P .. rows_pad - 1 are zeros.  A thread writes one 16-B vector of 8 consecutive columns.
+template <bool kF32>
+__global__ void __launch_bounds__(kThreads) vit_patchify_kernel(const void* __restrict__ pix, uint4* __restrict__ out,
+                                                                long long rows_real, long long rows_pad, int kvec, int C, int H,
+                                                                int W, int p, int P) {
+    const size_t total = (size_t)rows_pad * kvec, stride = (size_t)gridDim.x * blockDim.x;
+    const int gw = W / p;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const long long r = (long long)(i / kvec);
+        const int cv = (int)(i - (size_t)r * kvec);
+        float f[8];
+        if (r < rows_real) {
+            const long long b = r / P;
+            const int patch = (int)(r - b * P), hi = patch / gw, wi = patch - (patch / gw) * gw;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const int col = cv * 8 + k, c = col % C, q = col / C, p2 = q % p, p1 = q / p;
+                const size_t idx = ((size_t)(b * C + c) * H + (size_t)(hi * p + p1)) * W + (size_t)(wi * p + p2);
+                f[k] = kF32 ? __ldg(reinterpret_cast<const float*>(pix) + idx)
+                            : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(pix)[idx]);
+            }
+        } else {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) f[k] = 0.f;
+        }
+        st16(out + i, pack8(f));
+    }
+}
+
+// y [s_run, b, h]: row 0 = cls + pos[0]; row s in 1..P = patch[bi * P + s - 1] + (bias + pos[s]); rows > P zero.  fp32 math, one
+// rounding to bf16; with kDrop the dropout of bg_dropout_add_fwd at (token s, sample sample_base + bi) is applied before it.
+// grid = (column blocks, row groups over s); a thread owns one 8-column vector of every sample of its rows.
+template <bool kDrop>
+__global__ void __launch_bounds__(kThreads) vit_embed_fwd_kernel(const uint4* __restrict__ patch, const uint4* __restrict__ bias,
+                                                                 const uint4* __restrict__ cls, const uint4* __restrict__ pos,
+                                                                 uint4* __restrict__ y, long long b, long long P, long long s_run,
+                                                                 int nvec, DropoutCoords d) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= nvec) return;
+    float bv[8], cv[8];
+    unpack8(__ldg(bias + c), bv);
+    unpack8(__ldg(cls + c), cv);
+    for (long long s = blockIdx.y; s < s_run; s += gridDim.y) {
+        if (s > P) {
+            for (long long bi = 0; bi < b; ++bi) st16(y + (size_t)(s * b + bi) * nvec + c, make_uint4(0u, 0u, 0u, 0u));
+            continue;
+        }
+        float base[8];
+        unpack8(__ldg(pos + (size_t)s * nvec + c), base);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) base[k] = __fadd_rn(base[k], s == 0 ? cv[k] : bv[k]);
+#pragma unroll 4
+        for (long long bi = 0; bi < b; ++bi) {
+            const long long r = s * b + bi;
+            float f[8];
+            if (s == 0) {
+#pragma unroll
+                for (int k = 0; k < 8; ++k) f[k] = base[k];
+            } else {
+                unpack8(ld16_stream(patch + (size_t)(bi * P + s - 1) * nvec + c), f);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) f[k] = __fadd_rn(f[k], base[k]);
+            }
+            if (kDrop) {
+                const unsigned keep = dropout_keep8(d, r, c);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) f[k] = (keep >> k) & 1u ? __fmul_rn(f[k], d.scale) : 0.f;
+            }
+            st16(y + (size_t)r * nvec + c, pack8(f));
+        }
+    }
+}
+
+// backward of the above: g = (keep * scale *) dy.  dpatch[bi * P + s - 1] = bf16(g[s, bi]) for s in 1..P, rows b*P .. rows_pad - 1
+// zero; dpos[s] = fp32 sum over the samples in order of g[s, bi] for s < P + 1 (dpos[0] is also dcls); dbias_partial[blockIdx.y] =
+// the CTA's fp32 sum of dpos rows 1..P in row order.  Rows > P of dy belong to padding tokens and are not read.
+template <bool kDrop>
+__global__ void __launch_bounds__(kThreads) vit_embed_bwd_kernel(const uint4* __restrict__ dy, uint4* __restrict__ dpatch,
+                                                                 float* __restrict__ dpos, float* __restrict__ dbias_partial,
+                                                                 long long b, long long P, long long rows_pad, int nvec,
+                                                                 DropoutCoords d) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= nvec) return;
+    float accb[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) accb[k] = 0.f;
+    for (long long s = blockIdx.y; s <= P; s += gridDim.y) {
+        float acc[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) acc[k] = 0.f;
+#pragma unroll 4
+        for (long long bi = 0; bi < b; ++bi) {
+            const long long r = s * b + bi;
+            float g[8];
+            unpack8(ld16_stream(dy + (size_t)r * nvec + c), g);
+            if (kDrop) {
+                const unsigned keep = dropout_keep8(d, r, c);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) g[k] = (keep >> k) & 1u ? __fmul_rn(g[k], d.scale) : 0.f;
+            }
+#pragma unroll
+            for (int k = 0; k < 8; ++k) acc[k] = __fadd_rn(acc[k], g[k]);
+            if (s > 0) st16(dpatch + (size_t)(bi * P + s - 1) * nvec + c, pack8(g));
+        }
+        float4* dp = reinterpret_cast<float4*>(dpos + ((size_t)s * nvec + c) * 8);
+        dp[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+        dp[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+        if (s > 0) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) accb[k] = __fadd_rn(accb[k], acc[k]);
+        }
+    }
+    if (blockIdx.y == 0)
+        for (long long r = b * P; r < rows_pad; ++r) st16(dpatch + (size_t)r * nvec + c, make_uint4(0u, 0u, 0u, 0u));
+    float4* p = reinterpret_cast<float4*>(dbias_partial + ((size_t)blockIdx.y * nvec + c) * 8);
+    p[0] = make_float4(accb[0], accb[1], accb[2], accb[3]);
+    p[1] = make_float4(accb[4], accb[5], accb[6], accb[7]);
+}
+
+// the ViT pooler's activation (vit_hf pooler: dense + tanh):  y = tanh(x + b);  backward: dx = dy * (1 - tanh(x + b)^2)
+template <bool kBackward>
+__global__ void __launch_bounds__(kThreads) bias_tanh_kernel(const uint4* __restrict__ x, const uint4* __restrict__ bias,
+                                                             const uint4* __restrict__ dy, uint4* __restrict__ out, long long rows,
+                                                             int cvec) {
+    const size_t total = (size_t)rows * cvec, stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const size_t c = i % cvec;
+        float f[8], b[8];
+        unpack8(ld16_stream(x + i), f);
+        if (bias != nullptr) {
+            unpack8(__ldg(bias + c), b);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) f[k] += b[k];
+        }
+        if (kBackward) {
+            float g[8];
+            unpack8(ld16_stream(dy + i), g);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const float t = tanhf(f[k]);
+                f[k] = g[k] * (1.f - t * t);
+            }
+        } else {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) f[k] = tanhf(f[k]);
+        }
+        st16(out + i, pack8(f));
+    }
+}
+
 }  // namespace
 
 #define BG_ALIGNED16(p) (((uintptr_t)(p) % 16) == 0)
@@ -1031,6 +1186,108 @@ extern "C" int bg_dropout_bwd(const void* dy, void* dx, float* dbias_partial, in
     return BG_OK;
 }
 
+extern "C" int bg_vit_patchify(const void* pixels, int pixel_dtype, void* out, long long batch, long long channels, long long height,
+                               long long width, long long patch, long long rows_pad, void* stream) {
+    const char* who = "bg_vit_patchify";
+    if (pixel_dtype != BG_BF16 && pixel_dtype != BG_F32) return fail(BG_EUNSUPPORTED, "%s: pixel dtype %d", who, pixel_dtype);
+    if (batch < 1 || channels < 1 || patch < 1 || height < patch || width < patch || height % patch || width % patch)
+        return fail(BG_EINVAL, "%s: image %lldx%lldx%lld x %lld does not split into %lldx%lld patches", who, batch, channels, height, width,
+                    patch, patch);
+    const long long k = patch * patch * channels, P = (height / patch) * (width / patch);
+    if (k % 8) return fail(BG_EINVAL, "%s: patch row p*p*C = %lld must be a multiple of 8", who, k);
+    if (rows_pad < batch * P || rows_pad % 8) return fail(BG_EINVAL, "%s: rows_pad %lld must be a multiple of 8 >= B*P = %lld", who, rows_pad, batch * P);
+    if (batch * channels * height * width > (1LL << 40) || k > (1LL << 24)) return fail(BG_EUNSUPPORTED, "%s: image too large", who);
+    const size_t esz = pixel_dtype == BG_F32 ? 4 : 2;
+    if ((uintptr_t)pixels % esz || !BG_ALIGNED16(out)) return fail(BG_EINVAL, "%s: alignment", who);
+    const int grid = local_grid((size_t)rows_pad * (k / 8), kThreads);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (pixel_dtype == BG_F32)
+        vit_patchify_kernel<true><<<grid, kThreads, 0, st>>>(pixels, (uint4*)out, batch * P, rows_pad, (int)(k / 8), (int)channels,
+                                                             (int)height, (int)width, (int)patch, (int)P);
+    else
+        vit_patchify_kernel<false><<<grid, kThreads, 0, st>>>(pixels, (uint4*)out, batch * P, rows_pad, (int)(k / 8), (int)channels,
+                                                              (int)height, (int)width, (int)patch, (int)P);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+// shared checks of the two embedding entries: shapes (the dropout arguments as bg_dropout_add_fwd's, over s_run x batch rows)
+static int vit_embed_args(long long batch, long long n_patches, long long s_run, long long h, long long sample_base, double p,
+                          unsigned seed, unsigned iteration, unsigned site, DropoutCoords* d, const char* who) {
+    if (batch < 1 || n_patches < 1 || s_run < n_patches + 1)
+        return fail(BG_EINVAL, "%s: batch %lld, patches %lld and s_run %lld must satisfy batch >= 1, s_run > patches >= 1", who, batch,
+                    n_patches, s_run);
+    return dropout_args(s_run * batch, h, batch, 0, sample_base, p, seed, iteration, site, d, who);
+}
+
+// threads of a (column blocks, row groups) launch: one thread per 8-column vector, at most kThreads per CTA
+static dim3 vit_block(long long nvec) {
+    const long long t = (nvec + 31) / 32 * 32;
+    return dim3((unsigned)(t < kThreads ? t : kThreads), 1, 1);
+}
+
+extern "C" int bg_vit_embed_fwd(const void* patch_out, const void* bias, const void* cls, const void* pos, void* y, long long batch,
+                                long long n_patches, long long s_run, long long h, long long sample_base, double p, unsigned seed,
+                                unsigned iteration, unsigned site, void* stream) {
+    DropoutCoords d;
+    int rc = vit_embed_args(batch, n_patches, s_run, h, sample_base, p, seed, iteration, site, &d, "bg_vit_embed_fwd");
+    if (rc) return rc;
+    if (patch_out == nullptr || bias == nullptr || cls == nullptr || pos == nullptr || y == nullptr || !BG_ALIGNED16(patch_out) ||
+        !BG_ALIGNED16(bias) || !BG_ALIGNED16(cls) || !BG_ALIGNED16(pos) || !BG_ALIGNED16(y))
+        return fail(BG_EINVAL, "bg_vit_embed_fwd: pointers must be non-null and 16-B aligned");
+    const long long nvec = h / 8;
+    const dim3 block = vit_block(nvec);
+    long long gy = g_tun.local_ctas / ((nvec + block.x - 1) / block.x);
+    gy = gy < 1 ? 1 : (gy > s_run ? s_run : gy);
+    const dim3 grid((unsigned)((nvec + block.x - 1) / block.x), (unsigned)(gy > 65535 ? 65535 : gy), 1);
+    cudaStream_t st = (cudaStream_t)stream;
+    const uint4 *pv = (const uint4*)patch_out, *bv = (const uint4*)bias, *cv = (const uint4*)cls, *qv = (const uint4*)pos;
+    if (p > 0.0) vit_embed_fwd_kernel<true><<<grid, block, 0, st>>>(pv, bv, cv, qv, (uint4*)y, batch, n_patches, s_run, (int)nvec, d);
+    else vit_embed_fwd_kernel<false><<<grid, block, 0, st>>>(pv, bv, cv, qv, (uint4*)y, batch, n_patches, s_run, (int)nvec, d);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_vit_embed_bwd(const void* dy, void* dpatch, float* dpos, float* dbias_partial, int n_partial, long long batch,
+                                long long n_patches, long long s_run, long long rows_pad, long long h, long long sample_base, double p,
+                                unsigned seed, unsigned iteration, unsigned site, void* stream) {
+    DropoutCoords d;
+    int rc = vit_embed_args(batch, n_patches, s_run, h, sample_base, p, seed, iteration, site, &d, "bg_vit_embed_bwd");
+    if (rc) return rc;
+    if (rows_pad < batch * n_patches || rows_pad % 8)
+        return fail(BG_EINVAL, "bg_vit_embed_bwd: rows_pad %lld must be a multiple of 8 >= batch x patches = %lld", rows_pad, batch * n_patches);
+    if (n_partial < 1 || n_partial > 65535) return fail(BG_EINVAL, "bg_vit_embed_bwd: n_partial %d must be in [1, 65535]", n_partial);
+    if (dy == nullptr || dpatch == nullptr || dpos == nullptr || dbias_partial == nullptr || !BG_ALIGNED16(dy) || !BG_ALIGNED16(dpatch) ||
+        !BG_ALIGNED16(dpos) || !BG_ALIGNED16(dbias_partial))
+        return fail(BG_EINVAL, "bg_vit_embed_bwd: pointers must be non-null and 16-B aligned");
+    const long long nvec = h / 8;
+    const dim3 block = vit_block(nvec);
+    const dim3 grid((unsigned)((nvec + block.x - 1) / block.x), (unsigned)n_partial, 1);
+    cudaStream_t st = (cudaStream_t)stream;
+    // (every one of the n_partial row groups writes its dbias partial, zeros if it visits no row)
+    if (p > 0.0)
+        vit_embed_bwd_kernel<true><<<grid, block, 0, st>>>((const uint4*)dy, (uint4*)dpatch, dpos, dbias_partial, batch, n_patches, rows_pad,
+                                                           (int)nvec, d);
+    else
+        vit_embed_bwd_kernel<false><<<grid, block, 0, st>>>((const uint4*)dy, (uint4*)dpatch, dpos, dbias_partial, batch, n_patches,
+                                                            rows_pad, (int)nvec, d);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_bias_tanh(const void* x, const void* bias, const void* dy, void* out, long long rows, long long cols, void* stream) {
+    if (cols <= 0 || cols % 8) return fail(BG_EINVAL, "bg_bias_tanh: cols %lld must be a positive multiple of 8", cols);
+    if (rows < 0) return fail(BG_EINVAL, "bg_bias_tanh: rows %lld must be >= 0", rows);
+    if (!BG_ALIGNED16(x) || !BG_ALIGNED16(bias) || !BG_ALIGNED16(dy) || !BG_ALIGNED16(out)) return fail(BG_EINVAL, "bg_bias_tanh: 16-B alignment");
+    if (rows == 0) return BG_OK;
+    const int grid = local_grid((size_t)rows * cols / 8, kThreads);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dy == nullptr) bias_tanh_kernel<false><<<grid, kThreads, 0, st>>>((const uint4*)x, (const uint4*)bias, nullptr, (uint4*)out, rows, (int)(cols / 8));
+    else bias_tanh_kernel<true><<<grid, kThreads, 0, st>>>((const uint4*)x, (const uint4*)bias, (const uint4*)dy, (uint4*)out, rows, (int)(cols / 8));
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
 // loads every kernel of this file up front (see bg_preload_coll in bg_coll.cu)
 int bg_preload_ops() {
 #define K(f) reinterpret_cast<const void*>(&f)
@@ -1040,7 +1297,10 @@ int bg_preload_ops() {
                              K((bias_gelu_kernel<false, true>)), K(swiglu_fwd_kernel), K(swiglu_bwd_kernel), K(qkv_rope_kernel),
                              K(ce_rowmax_kernel<true>), K(ce_rowmax_kernel<false>), K(ce_sumexp_kernel<true>), K(ce_sumexp_kernel<false>),
                              K(ce_bwd_kernel<true>), K(ce_bwd_kernel<false>), K(dropout_add_fwd_kernel<true>),
-                             K(dropout_add_fwd_kernel<false>), K(dropout_bwd_kernel)};
+                             K(dropout_add_fwd_kernel<false>), K(dropout_bwd_kernel), K(vit_patchify_kernel<true>),
+                             K(vit_patchify_kernel<false>), K(vit_embed_fwd_kernel<true>), K(vit_embed_fwd_kernel<false>),
+                             K(vit_embed_bwd_kernel<true>), K(vit_embed_bwd_kernel<false>), K(bias_tanh_kernel<true>),
+                             K(bias_tanh_kernel<false>)};
 #undef K
     for (const void* k : kernels) {
         cudaFuncAttributes attr;

@@ -268,6 +268,35 @@ int bg_dropout_add_fwd(const void* x, const void* bias, int bias_dtype, const vo
 int bg_dropout_bwd(const void* dy, void* dx, float* dbias_partial, int n_partial, long long rows, long long h, long long b_loc,
                    long long seq_base, long long sample_base, double p, unsigned seed, unsigned iteration, unsigned site,
                    void* stream);
+/* ViT front end (vit_hf/ViTModel_sequential.py ViTEmbeddings_).  bg_vit_patchify: pixels [batch][channels][height][width] (BG_BF16
+ * or BG_F32) -> bf16 patch rows out [rows_pad][patch * patch * channels] in einops' "b c (h p1) (w p2) -> b (h w) (p1 p2 c)" order
+ * (fp32 pixels rounded once, RNE); rows batch * P .. rows_pad - 1 are zeros, P = (height / patch) * (width / patch).
+ * BG_EUNSUPPORTED for another pixel dtype; BG_EINVAL for an image that does not split into patches, patch * patch * channels not a
+ * multiple of 8, rows_pad not a multiple of 8 >= batch * P, pixels not aligned to their element size or out not 16-B aligned. */
+int bg_vit_patchify(const void* pixels, int pixel_dtype, void* out, long long batch, long long channels, long long height,
+                    long long width, long long patch, long long rows_pad, void* stream);
+/* y [s_run][batch][h] bf16 (SBH) from the patch GEMM's output patch_out [>= batch * n_patches][h] (row bi * n_patches + j = patch j
+ * of sample bi) and bf16 [h] bias, [h] cls, [n_patches + 1][h] pos:  row 0 = cls + pos[0]; row s in 1..n_patches =
+ * patch_out[bi * n_patches + s - 1] + (bias + pos[s]); rows n_patches + 1 .. s_run - 1 (padding tokens) = 0.  fp32 math, one rounding
+ * per step.  p > 0: the embedding dropout applied to each sum before its rounding, with exactly bg_dropout_add_fwd's mask at (token s,
+ * sample sample_base + bi, seed, iteration, site) and scale.  BG_EINVAL for batch < 1, n_patches < 1, s_run <= n_patches, a null or
+ * non-16-B-aligned pointer, and the dropout arguments bg_dropout_add_fwd rejects (h, p, coordinates). */
+int bg_vit_embed_fwd(const void* patch_out, const void* bias, const void* cls, const void* pos, void* y, long long batch,
+                     long long n_patches, long long s_run, long long h, long long sample_base, double p, unsigned seed, unsigned iteration,
+                     unsigned site, void* stream);
+/* its backward from dy [s_run][batch][h] (g = dy, or keep * scale * dy regenerated from the same coordinates when p > 0):
+ * dpatch [rows_pad][h] bf16 = g of rows 1..n_patches in (sample, patch) order, rows batch * n_patches .. rows_pad - 1 zero;
+ * dpos [n_patches + 1][h] fp32 = the sums over the samples, in sample order, of g at each token (row 0 is also the CLS token's
+ * gradient); dbias_partial [n_partial][h] fp32 = per-row-group sums of dpos rows 1..n_patches, in row order (the caller adds the
+ * n_partial rows).  The sums depend on n_partial only, so the result is deterministic.  Rows of padding tokens are not read.
+ * BG_EINVAL as the forward, and for rows_pad not a multiple of 8 >= batch * n_patches and n_partial outside [1, 65535]. */
+int bg_vit_embed_bwd(const void* dy, void* dpatch, float* dpos, float* dbias_partial, int n_partial, long long batch,
+                     long long n_patches, long long s_run, long long rows_pad, long long h, long long sample_base, double p, unsigned seed,
+                     unsigned iteration, unsigned site, void* stream);
+/* bias + tanh of the ViT pooler: out = tanh(x + bias) when dy == NULL, else out = dy * (1 - tanh(x + bias)^2), fp32 math, one
+ * rounding.  bias may be NULL; the dbias column sums are the caller's, as for bg_bias_gelu.  BG_EINVAL for rows < 0, cols not a
+ * positive multiple of 8 or a pointer not 16-B aligned. */
+int bg_bias_tanh(const void* x, const void* bias, const void* dy, void* out, long long rows, long long cols, void* stream);
 /* host-only: one Philox4x32-10 block (the generator of curand_philox4x32_x.h), so the mask definition can be checked without a
  * GPU.  No CUDA call. */
 void bg_philox4x32_10(const uint32_t ctr[4], const uint32_t key[2], uint32_t out[4]);
