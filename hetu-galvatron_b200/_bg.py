@@ -94,6 +94,16 @@ SIGNATURES = {
     "bg_vit_embed_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _c.c_double, _c.c_uint, _c.c_uint, _c.c_uint, _vp]),
     "bg_vit_embed_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _ll, _ll, _ll, _ll, _ll, _ll, _c.c_double, _c.c_uint, _c.c_uint, _c.c_uint, _vp]),
     "bg_bias_tanh": (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _vp]),
+    "bg_swin_window_qkv_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
+    "bg_swin_window_qkv_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
+    "bg_swin_window_merge_fwd": (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
+    "bg_swin_window_merge_bwd": (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
+    "bg_swin_merge_ln_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _i, _ll, _ll, _ll, _f, _vp]),
+    "bg_swin_merge_ln_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _ll, _ll, _ll, _ll, _i, _ll, _ll, _vp]),
+    "bg_swin_mean_pool_fwd": (_i, [_vp, _vp, _ll, _ll, _ll, _ll, _ll, _vp]),
+    "bg_swin_mean_pool_bwd": (_i, [_vp, _vp, _ll, _ll, _ll, _ll, _vp]),
+    "bg_drop_path_add_fwd": (_i, [_vp, _vp, _i, _vp, _vp, _ll, _ll, _ll, _ll, _c.c_double, _c.c_uint, _c.c_uint, _c.c_uint, _vp]),
+    "bg_drop_path_add_bwd": (_i, [_vp, _vp, _vp, _i, _ll, _ll, _ll, _ll, _c.c_double, _c.c_uint, _c.c_uint, _c.c_uint, _vp]),
     "bg_philox4x32_10": (None, [_c.POINTER(_c.c_uint32), _c.POINTER(_c.c_uint32), _c.POINTER(_c.c_uint32)]),
     "bg_swiglu_fwd": (_i, [_vp, _vp, _ll, _ll, _vp]),
     "bg_swiglu_bwd": (_i, [_vp, _vp, _vp, _ll, _ll, _vp]),

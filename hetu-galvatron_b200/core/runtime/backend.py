@@ -772,6 +772,106 @@ class CudaBackend:
                                                      int(sample_base), float(p), int(seed), int(iteration), int(site), _s()))
         return dpatch, dpos[0], dpos, dbp.sum(0)
 
+    # ---- Swin: window relayouts through a token map (map[w * L + i] = token at position i of window w, inv its inverse; int32 on
+    # the device), patch merging + LayerNorm, mean-pool and per-sample drop path (include/bg_galvatron.h)
+    def swin_window_qkv_fwd(self, mixed, bias, tmap, inv, n_windows, mb, heads, hn):
+        """mixed [T_run * mb, heads * 3 * hn] SBH rows + bias -> q, k, v [mb * n_windows, L, heads, hn]."""
+        L = tmap.numel() // n_windows
+        q, k, v = [torch.empty(mb * n_windows, L, heads, hn, dtype=mixed.dtype, device=mixed.device) for _ in range(3)]
+        self.bg.check(self.bg.lib().bg_swin_window_qkv_fwd(_p(mixed), _p(bias), _p(tmap), _p(q), _p(k), _p(v), mb, tmap.numel(),
+                                                           mixed.numel() // (mb * heads * 3 * hn), n_windows, L, heads, hn, _s()))
+        return q, k, v
+
+    def swin_window_qkv_bwd(self, dq, dk, dv, tmap, inv, n_windows, mb, t_run):
+        """-> (dmixed [t_run * mb, heads * 3 * hn] with zero padding-token rows, dbias [heads * 3 * hn] fp32)."""
+        heads, hn = dq.shape[2], dq.shape[3]
+        dmixed = torch.empty(t_run * mb, heads * 3 * hn, dtype=dq.dtype, device=dq.device)
+        npart = min(self.norm_partials, t_run * mb)
+        dbp = torch.empty(npart, heads * 3 * hn, dtype=torch.float32, device=dq.device)
+        self.bg.check(self.bg.lib().bg_swin_window_qkv_bwd(_p(dq.contiguous()), _p(dk.contiguous()), _p(dv.contiguous()), _p(dmixed), _p(dbp),
+                                                           npart, _p(inv), mb, tmap.numel(), t_run, n_windows, tmap.numel() // n_windows,
+                                                           heads, hn, _s()))
+        return dmixed, dbp.sum(0)
+
+    def swin_window_merge_fwd(self, windows, tmap, inv, n_windows, mb, t_run):
+        """attention output [mb * n_windows, L, heads, hn] -> SBH rows [t_run, mb, heads * hn], padding-token rows zero."""
+        windows = windows.contiguous()
+        cols = windows.shape[2] * windows.shape[3]
+        rows = torch.empty(t_run, mb, cols, dtype=windows.dtype, device=windows.device)
+        self.bg.check(self.bg.lib().bg_swin_window_merge_fwd(_p(windows), _p(rows), _p(tmap), _p(inv), mb, tmap.numel(), t_run, n_windows,
+                                                             tmap.numel() // n_windows, cols, _s()))
+        return rows
+
+    def swin_window_merge_bwd(self, drows, tmap, inv, n_windows, mb, heads, hn):
+        drows = drows.contiguous()
+        L = tmap.numel() // n_windows
+        dwin = torch.empty(mb * n_windows, L, heads, hn, dtype=drows.dtype, device=drows.device)
+        self.bg.check(self.bg.lib().bg_swin_window_merge_bwd(_p(drows), _p(dwin), _p(tmap), _p(inv), mb, tmap.numel(),
+                                                             drows.numel() // (mb * heads * hn), n_windows, L, heads * hn, _s()))
+        return dwin
+
+    def swin_merge_ln_fwd(self, x, add_bias, weight, bias, eps, mb, height, width, r, in_bsh, t_out_run):
+        """x: the height x width grid of mb samples (SBH rows, or with ``in_bsh`` the patch GEMM's (sample, patch) rows), C columns ->
+        (y [t_out_run, mb, r * r * C] with zero padding-token rows, mean, rstd)."""
+        x = x.contiguous()
+        c = x.shape[-1]
+        y = torch.empty(t_out_run, mb, r * r * c, dtype=x.dtype, device=x.device)
+        mean = torch.empty(t_out_run * mb, dtype=torch.float32, device=x.device)
+        rstd = torch.empty_like(mean)
+        self.bg.check(self.bg.lib().bg_swin_merge_ln_fwd(_p(x), _p(add_bias) if add_bias is not None else None, _p(weight), _p(bias), _p(y),
+                                                         _p(mean), _p(rstd), mb, height, width, r, 1 if in_bsh else 0, x.numel() // c, c,
+                                                         t_out_run, float(eps), _s()))
+        return y, mean, rstd
+
+    def swin_merge_ln_bwd(self, dy, x, add_bias, weight, mean, rstd, mb, height, width, r, in_bsh):
+        """-> (dx in x's layout, zero past the real rows; dweight, dbias of the norm; d(add_bias) fp32 or None)."""
+        x, dy = x.contiguous(), dy.contiguous()
+        c = x.shape[-1]
+        dx = torch.empty_like(x)
+        npart = min(self.norm_partials, max(1, mb * (height // r) * (width // r)))
+        dwp = torch.empty(npart, r * r * c, dtype=torch.float32, device=x.device)
+        dbp = torch.empty_like(dwp)
+        dap = torch.empty_like(dwp) if add_bias is not None else None
+        self.bg.check(self.bg.lib().bg_swin_merge_ln_bwd(_p(dy), _p(x), _p(add_bias) if add_bias is not None else None, _p(weight), _p(mean),
+                                                         _p(rstd), _p(dx), _p(dwp), _p(dbp), _p(dap) if dap is not None else None, npart, mb,
+                                                         height, width, r, 1 if in_bsh else 0, x.numel() // c, c, _s()))
+        return dx, dwp.sum(0).to(weight.dtype), dbp.sum(0).to(weight.dtype), (dap.sum(0) if dap is not None else None)
+
+    def swin_mean_pool_fwd(self, x, tokens, rows_out):
+        """x [t_run, mb, C] -> [rows_out, C]: the mean of the first ``tokens`` tokens of each sample, zero rows past mb."""
+        x = x.contiguous()
+        t_run, mb, c = x.shape
+        y = torch.empty(rows_out, c, dtype=x.dtype, device=x.device)
+        self.bg.check(self.bg.lib().bg_swin_mean_pool_fwd(_p(x), _p(y), tokens, t_run, mb, rows_out, c, _s()))
+        return y
+
+    def swin_mean_pool_bwd(self, dy, tokens, t_run, mb):
+        dy = dy.contiguous()
+        dx = torch.empty(t_run, mb, dy.shape[-1], dtype=dy.dtype, device=dy.device)
+        self.bg.check(self.bg.lib().bg_swin_mean_pool_bwd(_p(dy), _p(dx), tokens, t_run, mb, dy.shape[-1], _s()))
+        return dx
+
+    def drop_path_add_fwd(self, x, bias, residual, p, seed, iteration, site, sample_base):
+        """y = residual + keep_b * scale * (x + bias) on an SBH tensor x [s, b, h] of samples sample_base..; bias [h] bf16 / fp32."""
+        s, b, h = x.shape
+        x, residual = x.contiguous(), residual.contiguous()
+        y = torch.empty_like(x)
+        bcode = self.bg.dtype_code(bias.dtype) if bias is not None else 0
+        self.bg.check(self.bg.lib().bg_drop_path_add_fwd(_p(x), _p(bias) if bias is not None else None, bcode, _p(residual), _p(y), s * b, h,
+                                                         b, int(sample_base), float(p), int(seed), int(iteration), int(site), _s()))
+        return y
+
+    def drop_path_add_bwd(self, dy, p, seed, iteration, site, sample_base, with_bias):
+        """-> (dx = keep_b * scale * dy, its fp32 column sums or None)."""
+        s, b, h = dy.shape
+        dy = dy.contiguous()
+        dx = torch.empty_like(dy)
+        npart = min(self.norm_partials, max(1, s * b))
+        dbp = torch.empty(npart, h, dtype=torch.float32, device=dy.device) if with_bias else None
+        self.bg.check(self.bg.lib().bg_drop_path_add_bwd(_p(dy), _p(dx), _p(dbp) if dbp is not None else None, npart, s * b, h, b,
+                                                         int(sample_base), float(p), int(seed), int(iteration), int(site), _s()))
+        return dx, (dbp.sum(0) if dbp is not None else None)
+
     def dropout_add_fwd(self, x, bias, residual, p, seed, iteration, site, seq_base, sample_base):
         """y = residual + keep * scale * (x + bias) on an SBH tensor x [s_loc, b_loc, h] whose rows are tokens seq_base.. of samples
         sample_base.. (mask: include/bg_galvatron.h).  bias [h] (bf16 / fp32) and residual (x's shape) may be None."""
@@ -843,7 +943,7 @@ class CudaBackend:
         # the reference casts cos/sin to the activation dtype before applying them (apply_rotary_pos_emb)
         return torch.cos(freqs).to(dtype).float().contiguous(), torch.sin(freqs).to(dtype).float().contiguous()
 
-    def attention(self, q, k, v, causal, softmax_scale, key_mask=None, dropout_p=0.0):
+    def attention(self, q, k, v, causal, softmax_scale, key_mask=None, dropout_p=0.0, window_mask=None):
         """Attention is a LIBRARY call, as in the reference (transformer.py:495 calls flash-attn; K3 is not a collective and
         is outside the hot-path scope).  The default is cuDNN's fused SDPA, reached
         through torch SDPA; HGB_ATTN=flash selects flash-attn 2.  q [b,s,n,d], k/v [b,s,ng,d] (GQA un-expanded).  Differentiable.
@@ -852,6 +952,13 @@ class CudaBackend:
         cuDNN's."""
         import torch.nn.functional as F
         from torch.nn.attention import SDPBackend, sdpa_kernel
+        if window_mask is not None:
+            # Swin's shifted windows: an additive [windows, 1, L, L] mask (0 / -inf, q's dtype), one row of windows per sample
+            assert not causal and key_mask is None and dropout_p == 0.0
+            with sdpa_kernel([SDPBackend.CUDNN_ATTENTION, SDPBackend.EFFICIENT_ATTENTION, SDPBackend.MATH]):
+                o = F.scaled_dot_product_attention(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), attn_mask=window_mask,
+                                                   scale=softmax_scale)
+            return o.transpose(1, 2)
         if key_mask is not None:
             # BERT's padding mask (bert_hf/BertModel_sequential.py: get_extended_attention_mask): key j of sample b is visible iff
             # key_mask[b, j]; fused SDPA with an additive mask (cuDNN where it accepts the mask, the memory-efficient kernel else)

@@ -29,6 +29,9 @@ _CTX = DropoutContext(seed=0, iteration=0, sample_base=0, batch=None)
 _STEP = dict(seed=0, iteration=0, sample_base=0)
 
 SITE_EMBEDDING, SITE_ATTENTION, SITE_MLP = 0, 1, 2
+# Swin's per-sample drop path on the attention branch (its blocks have no hidden dropout there; the mask's counter is one no
+# dropout element uses, include/bg_galvatron.h bg_drop_path_add_fwd)
+SITE_DROP_PATH = SITE_ATTENTION
 
 
 def check_probability(p, name="dropout"):

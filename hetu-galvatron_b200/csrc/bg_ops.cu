@@ -915,6 +915,374 @@ __global__ void __launch_bounds__(kThreads) bias_tanh_kernel(const uint4* __rest
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Swin (swin/SwinModel_tensor_parallel.py): the window relayouts around attention, patch merging + LayerNorm, the token mean-pool
+// and the per-sample drop path.  Activations are SBH rows (row = token * mb + sample) of tokens_run tokens per sample, the real
+// tokens first; a shifted window partition is one int32 token map per layer shape: map[w * L + i] = the token at position i of
+// window w (L = window * window tokens), and inv[t] = w * L + i its inverse.  Window rows are [mb * nW, L, ...], window
+// b * nW + w of sample b.
+// ---------------------------------------------------------------------------------------------
+// mixed [tokens_run * mb, heads * 3 * hn] (per head q | k | v, the fused QKV GEMM's layout) + bias -> q, k, v [mb * nW, L, heads, hn]
+// (one rounding).  A thread writes one 16-B vector; consecutive threads read consecutive vectors of one mixed row.
+__global__ void __launch_bounds__(kThreads) swin_window_qkv_fwd_kernel(const uint4* __restrict__ mixed, const uint4* __restrict__ bias,
+                                                                       const int* __restrict__ map, uint4* __restrict__ q,
+                                                                       uint4* __restrict__ k, uint4* __restrict__ v, long long mb,
+                                                                       long long nW, int L, int heads, int hv) {
+    const int ncol = heads * 3 * hv;
+    const size_t total = (size_t)mb * nW * L * ncol, stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const long long wrow = (long long)(i / ncol);
+        const int col = (int)(i - (size_t)wrow * ncol);
+        const long long wi = wrow / L, b = wi / nW;
+        const int pos = (int)(wrow - wi * L), w = (int)(wi - b * nW);
+        const long long src = (long long)__ldg(map + (size_t)w * L + pos) * mb + b;
+        const int h = col / (3 * hv), part = (col / hv) % 3, c = col % hv;
+        float f[8], bv[8];
+        unpack8(ld16_stream(mixed + (size_t)src * ncol + col), f);
+        unpack8(__ldg(bias + col), bv);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) f[e] = __fadd_rn(f[e], bv[e]);
+        uint4* dst = part == 0 ? q : (part == 1 ? k : v);
+        st16(dst + ((size_t)wrow * heads + h) * hv + c, pack8(f));
+    }
+}
+
+// its backward: dmixed rows gathered from dq, dk, dv through inv (padding-token rows zero); dbias_partial[blockIdx.y] = the CTA's
+// fp32 column sums in row order.  grid = (column blocks, row groups); a thread owns one column vector of every row it visits.
+__global__ void __launch_bounds__(kThreads) swin_window_qkv_bwd_kernel(const uint4* __restrict__ dq, const uint4* __restrict__ dk,
+                                                                       const uint4* __restrict__ dv, uint4* __restrict__ dmixed,
+                                                                       float* __restrict__ dbias_partial, const int* __restrict__ inv,
+                                                                       long long mb, long long T, long long T_run, long long nW, int L,
+                                                                       int heads, int hv) {
+    const int ncol = heads * 3 * hv;
+    const int col = blockIdx.x * blockDim.x + threadIdx.x;
+    if (col >= ncol) return;
+    const int h = col / (3 * hv), part = (col / hv) % 3, c = col % hv;
+    const uint4* src = part == 0 ? dq : (part == 1 ? dk : dv);
+    float acc[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e] = 0.f;
+    for (long long r = blockIdx.y; r < T_run * mb; r += gridDim.y) {
+        const long long t = r / mb, b = r - t * mb;
+        uint4 g = make_uint4(0u, 0u, 0u, 0u);
+        if (t < T) {
+            const int p = __ldg(inv + t), w = p / L, pos = p - w * L;
+            const long long wrow = (b * nW + w) * L + pos;
+            g = ld16_stream(src + ((size_t)wrow * heads + h) * hv + c);
+            float f[8];
+            unpack8(g, f);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) acc[e] = __fadd_rn(acc[e], f[e]);
+        }
+        st16(dmixed + (size_t)r * ncol + col, g);
+    }
+    float4* p = reinterpret_cast<float4*>(dbias_partial + ((size_t)blockIdx.y * ncol + col) * 8);
+    p[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    p[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+}
+
+// window rows [mb * nW, L, cvec vectors] <-> SBH rows [T_run * mb, cvec vectors], a pure copy.  Forward (window rows -> SBH):
+// SBH row t * mb + b reads window row (b * nW + w) * L + i with w * L + i = inv[t]; padding-token rows are zero.  Backward (SBH ->
+// window rows): window row (b * nW + w) * L + i reads SBH row map[w * L + i] * mb + b.  A thread writes one 16-B vector.
+template <bool kBackward>
+__global__ void __launch_bounds__(kThreads) swin_window_merge_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst,
+                                                                     const int* __restrict__ map, const int* __restrict__ inv,
+                                                                     long long mb, long long T, long long T_run, long long nW, int L,
+                                                                     int cvec) {
+    const size_t rows = kBackward ? (size_t)mb * nW * L : (size_t)T_run * mb;
+    const size_t total = rows * cvec, stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const long long r = (long long)(i / cvec);
+        const int c = (int)(i - (size_t)r * cvec);
+        long long s = -1;
+        if (kBackward) {
+            const long long wi = r / L, b = wi / nW;
+            const int pos = (int)(r - wi * L), w = (int)(wi - b * nW);
+            s = (long long)__ldg(map + (size_t)w * L + pos) * mb + b;
+        } else {
+            const long long t = r / mb, b = r - t * mb;
+            if (t < T) {
+                const int p = __ldg(inv + t), w = p / L;
+                s = (b * nW + w) * L + (p - w * L);
+            }
+        }
+        st16(dst + i, s < 0 ? make_uint4(0u, 0u, 0u, 0u) : ld16_stream(src + (size_t)s * cvec + c));
+    }
+}
+
+// Patch merging (r = 2) or the embedding's bias + norm (r = 1), then LayerNorm over the gathered row of r * r * C columns.  Output
+// row t' * mb + b (t' = (i', j') on the (H / r) x (W / r) grid) is the concatenation over q = 0..r*r-1 of input token
+// (r i' + (q & 1), r j' + (q >> 1)) of sample b -- HF's x0, x1, x2, x3 order -- plus add_bias when given, then
+// (v - mean) * rstd * w + b exactly as layernorm_fwd_kernel computes it (the same per-thread vectors, so the same rounding).
+// Input rows are SBH (token * mb + b) or, with in_bsh, (b * T_in + token) as the patch GEMM writes them.  Output rows of padding
+// tokens (t' >= T_out) are zero, with mean = rstd = 0.
+constexpr int kMergeVpt = 5;    // rows up to 256 * 8 * 5 = 10240 columns (Swin-H's widest merged row is 4 x 1280)
+struct MergeGeom {
+    long long mb, T_in, T_out, T_out_run;
+    int Wi, Wo, r, cvec_in, in_bsh;
+};
+__device__ __forceinline__ long long merge_src_row(const MergeGeom& g, long long to, long long b, int q) {
+    const long long io = to / g.Wo, jo = to - io * g.Wo;
+    const long long ts = (g.r * io + (q & 1)) * g.Wi + g.r * jo + (q >> 1);
+    return g.in_bsh ? b * g.T_in + ts : ts * g.mb + b;
+}
+
+template <bool kBias>
+__global__ void __launch_bounds__(kThreads) swin_merge_ln_fwd_kernel(const uint4* __restrict__ x, const uint4* __restrict__ add_bias,
+                                                                     const uint4* __restrict__ w, const uint4* __restrict__ bb,
+                                                                     uint4* __restrict__ y, float* __restrict__ mean_out,
+                                                                     float* __restrict__ rstd_out, MergeGeom g, float eps) {
+    __shared__ float smem[32];
+    const int nvec = g.r * g.r * g.cvec_in;
+    const float inv_n = 1.f / (float)(nvec * 8);
+    for (long long ro = blockIdx.x; ro < g.T_out_run * g.mb; ro += gridDim.x) {
+        const long long to = ro / g.mb, b = ro - to * g.mb;
+        if (to >= g.T_out) {
+            for (int v = threadIdx.x; v < nvec; v += kThreads) st16(y + ro * nvec + v, make_uint4(0u, 0u, 0u, 0u));
+            if (threadIdx.x == 0) { mean_out[ro] = 0.f; rstd_out[ro] = 0.f; }
+            continue;
+        }
+        float xf[kMergeVpt][8];
+        float s = 0.f;
+#pragma unroll
+        for (int j = 0; j < kMergeVpt; ++j) {
+            const int v = threadIdx.x + j * kThreads;
+            if (v < nvec) {
+                const int q = v / g.cvec_in, c = v - q * g.cvec_in;
+                unpack8(ld16_stream(x + (size_t)merge_src_row(g, to, b, q) * g.cvec_in + c), xf[j]);
+                if (kBias) {
+                    float bv[8];
+                    unpack8(__ldg(add_bias + v), bv);
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) xf[j][i] = __fadd_rn(xf[j][i], bv[i]);
+                }
+#pragma unroll
+                for (int i = 0; i < 8; ++i) s += xf[j][i];
+            }
+        }
+        const float mean = block_reduce<false>(s, smem) * inv_n;
+        float ss = 0.f;
+#pragma unroll
+        for (int j = 0; j < kMergeVpt; ++j) {
+            const int v = threadIdx.x + j * kThreads;
+            if (v < nvec) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) ss += (xf[j][i] - mean) * (xf[j][i] - mean);
+            }
+        }
+        const float rstd = rsqrtf(block_reduce<false>(ss, smem) * inv_n + eps);
+        if (threadIdx.x == 0) { mean_out[ro] = mean; rstd_out[ro] = rstd; }
+#pragma unroll
+        for (int j = 0; j < kMergeVpt; ++j) {
+            const int v = threadIdx.x + j * kThreads;
+            if (v < nvec) {
+                float f[8], gw[8], c[8];
+                unpack8(__ldg(w + v), gw);
+                unpack8(__ldg(bb + v), c);
+#pragma unroll
+                for (int i = 0; i < 8; ++i) f[i] = (xf[j][i] - mean) * rstd * gw[i] + c[i];
+                st16(y + ro * nvec + v, pack8(f));
+            }
+        }
+    }
+}
+
+// its backward, layernorm_bwd_kernel's math on the gathered row: dv = rstd * (g - mean(g) - vhat * mean(g * vhat)), g = dy * w,
+// scattered back to the r * r source rows (each input token feeds exactly one output token, so no two CTAs write one row).  The
+// output rows of padding tokens are not read; input rows mb * T_in .. rows_in - 1 get zeros.  Per-CTA fp32 partials: dw = sum
+// dy * vhat, db = sum dy, and with kBias dbias = sum dv (the column sums of the input gradient, before its rounding).
+template <int VPT, bool kBias>
+__global__ void __launch_bounds__(kThreads) swin_merge_ln_bwd_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x,
+                                                                     const uint4* __restrict__ add_bias, const uint4* __restrict__ w,
+                                                                     const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
+                                                                     uint4* __restrict__ dx, float* __restrict__ dw_partial,
+                                                                     float* __restrict__ db_partial, float* __restrict__ dbias_partial,
+                                                                     MergeGeom g, long long rows_in) {
+    __shared__ float smem[32];
+    const int nvec = g.r * g.r * g.cvec_in;
+    float dw[VPT][8], db[VPT][8], dbi[kBias ? VPT : 1][8];
+#pragma unroll
+    for (int j = 0; j < VPT; ++j)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { dw[j][i] = 0.f; db[j][i] = 0.f; if (kBias) dbi[j][i] = 0.f; }
+    const float inv_n = 1.f / (float)(nvec * 8);
+    for (long long ro = blockIdx.x; ro < g.T_out * g.mb; ro += gridDim.x) {
+        const long long to = ro / g.mb, b = ro - to * g.mb;
+        const float mean = mean_in[ro], rstd = rstd_in[ro];
+        float xh[VPT][8], gv[VPT][8];
+        float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+        for (int j = 0; j < VPT; ++j) {
+            const int v = threadIdx.x + j * kThreads;
+            if (v < nvec) {
+                const int q = v / g.cvec_in, c = v - q * g.cvec_in;
+                float wv[8];
+                unpack8(ld16_stream(x + (size_t)merge_src_row(g, to, b, q) * g.cvec_in + c), xh[j]);
+                unpack8(ld16_stream(dy + ro * nvec + v), gv[j]);
+                unpack8(__ldg(w + v), wv);
+                if (kBias) {
+                    float bv[8];
+                    unpack8(__ldg(add_bias + v), bv);
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) xh[j][i] = __fadd_rn(xh[j][i], bv[i]);
+                }
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    xh[j][i] = (xh[j][i] - mean) * rstd;
+                    dw[j][i] += gv[j][i] * xh[j][i];
+                    db[j][i] += gv[j][i];
+                    gv[j][i] *= wv[i];
+                    s1 += gv[j][i];
+                    s2 += gv[j][i] * xh[j][i];
+                }
+            }
+        }
+        s1 = block_reduce<false>(s1, smem) * inv_n;
+        s2 = block_reduce<false>(s2, smem) * inv_n;
+#pragma unroll
+        for (int j = 0; j < VPT; ++j) {
+            const int v = threadIdx.x + j * kThreads;
+            if (v < nvec) {
+                const int q = v / g.cvec_in, c = v - q * g.cvec_in;
+                float o[8];
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    o[i] = rstd * (gv[j][i] - s1 - xh[j][i] * s2);
+                    if (kBias) dbi[j][i] += o[i];
+                }
+                st16(dx + (size_t)merge_src_row(g, to, b, q) * g.cvec_in + c, pack8(o));
+            }
+        }
+    }
+    for (long long r = g.mb * g.T_in + blockIdx.x; r < rows_in; r += gridDim.x)
+        for (int c = threadIdx.x; c < g.cvec_in; c += kThreads) st16(dx + (size_t)r * g.cvec_in + c, make_uint4(0u, 0u, 0u, 0u));
+#pragma unroll
+    for (int j = 0; j < VPT; ++j) {
+        const int v = threadIdx.x + j * kThreads;
+        if (v < nvec) {
+            float4* d = reinterpret_cast<float4*>(dw_partial + ((size_t)blockIdx.x * nvec + v) * 8);
+            d[0] = make_float4(dw[j][0], dw[j][1], dw[j][2], dw[j][3]);
+            d[1] = make_float4(dw[j][4], dw[j][5], dw[j][6], dw[j][7]);
+            float4* e = reinterpret_cast<float4*>(db_partial + ((size_t)blockIdx.x * nvec + v) * 8);
+            e[0] = make_float4(db[j][0], db[j][1], db[j][2], db[j][3]);
+            e[1] = make_float4(db[j][4], db[j][5], db[j][6], db[j][7]);
+            if (kBias) {
+                float4* f = reinterpret_cast<float4*>(dbias_partial + ((size_t)blockIdx.x * nvec + v) * 8);
+                f[0] = make_float4(dbi[j][0], dbi[j][1], dbi[j][2], dbi[j][3]);
+                f[1] = make_float4(dbi[j][4], dbi[j][5], dbi[j][6], dbi[j][7]);
+            }
+        }
+    }
+}
+
+// Swin's pooler: y[b] = (sum over the first T tokens of x[t, b], fp32 in token order) / T for b < mb, zero rows up to rows_out.
+// Backward: dx[t, b] = dy[b] / T for t < T, zero for the padding tokens.  A thread owns one 16-B vector of output.
+template <bool kBackward>
+__global__ void __launch_bounds__(kThreads) swin_mean_pool_kernel(const uint4* __restrict__ in, uint4* __restrict__ out, long long T,
+                                                                  long long T_run, long long mb, long long rows_out, int cvec) {
+    const size_t rows = kBackward ? (size_t)T_run * mb : (size_t)rows_out;
+    const size_t total = rows * cvec, stride = (size_t)gridDim.x * blockDim.x;
+    const float tf = (float)T;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const long long r = (long long)(i / cvec);
+        const int c = (int)(i - (size_t)r * cvec);
+        float f[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) f[e] = 0.f;
+        if (kBackward) {
+            const long long t = r / mb;
+            if (t < T) {
+                unpack8(__ldg(in + (size_t)(r - t * mb) * cvec + c), f);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) f[e] = __fdiv_rn(f[e], tf);
+            }
+        } else if (r < mb) {
+            for (long long t = 0; t < T; ++t) {
+                float a[8];
+                unpack8(ld16_stream(in + ((size_t)t * mb + r) * cvec + c), a);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) f[e] = __fadd_rn(f[e], a[e]);
+            }
+#pragma unroll
+            for (int e = 0; e < 8; ++e) f[e] = __fdiv_rn(f[e], tf);
+        }
+        st16(out + i, pack8(f));
+    }
+}
+
+// Per-sample drop path of Swin's attention branch:  y = residual + keep_b * scale * (x + bias), dx = keep_b * scale * dy.  Row r
+// of a [rows, h] SBH block is sample sample_base + r % b_loc; the sample is kept iff word 0 of Philox4x32-10(ctr = (0, 0xffffffff,
+// sample, iteration), key = (seed, site)) >= threshold (token 0xffffffff: a counter no dropout element uses).  The arithmetic is
+// dropout_add_fwd_kernel's (__fadd_rn / __fmul_rn, one rounding at the end).
+__device__ __forceinline__ bool drop_path_keep(const DropoutCoords& d, long long r) {
+    const uint32_t smp = (uint32_t)(d.sample_base + r % d.b_loc);
+    return philox4x32_10(make_uint4(0u, 0xffffffffu, smp, d.iteration), make_uint2(d.seed, d.site)).x >= d.threshold;
+}
+
+template <bool kBiasF32>
+__global__ void __launch_bounds__(kThreads) drop_path_add_fwd_kernel(const uint4* __restrict__ x, const void* __restrict__ bias,
+                                                                     const uint4* __restrict__ residual, uint4* __restrict__ y,
+                                                                     long long rows, int nvec, DropoutCoords d) {
+    const int c = blockIdx.x * kThreads + threadIdx.x;
+    if (c >= nvec) return;
+    float bv[8];
+    if (bias == nullptr) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) bv[i] = 0.f;
+    } else if (kBiasF32) {
+        const float4* bp = reinterpret_cast<const float4*>(bias) + 2 * c;
+        const float4 b0 = __ldg(bp), b1 = __ldg(bp + 1);
+        bv[0] = b0.x; bv[1] = b0.y; bv[2] = b0.z; bv[3] = b0.w; bv[4] = b1.x; bv[5] = b1.y; bv[6] = b1.z; bv[7] = b1.w;
+    } else {
+        unpack8(__ldg(reinterpret_cast<const uint4*>(bias) + c), bv);
+    }
+    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
+        const size_t i = (size_t)r * nvec + c;
+        const bool keep = drop_path_keep(d, r);
+        float f[8], o[8];
+        unpack8(residual != nullptr ? ld16_stream(residual + i) : make_uint4(0u, 0u, 0u, 0u), o);
+        if (keep) {
+            unpack8(ld16_stream(x + i), f);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) o[k] = __fadd_rn(o[k], __fmul_rn(__fadd_rn(f[k], bv[k]), d.scale));
+        } else {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) o[k] = __fadd_rn(o[k], 0.f);
+        }
+        st16(y + i, pack8(o));
+    }
+}
+
+__global__ void __launch_bounds__(kThreads) drop_path_bwd_kernel(const uint4* __restrict__ dy, uint4* __restrict__ dx,
+                                                                 float* __restrict__ dbias_partial, long long rows, int nvec,
+                                                                 DropoutCoords d) {
+    const int c = blockIdx.x * kThreads + threadIdx.x;
+    if (c >= nvec) return;
+    float acc[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc[k] = 0.f;
+    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
+        const size_t i = (size_t)r * nvec + c;
+        float g[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) g[k] = 0.f;
+        if (drop_path_keep(d, r)) {
+            unpack8(ld16_stream(dy + i), g);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) g[k] = __fmul_rn(g[k], d.scale);
+        }
+#pragma unroll
+        for (int k = 0; k < 8; ++k) acc[k] = __fadd_rn(acc[k], g[k]);
+        st16(dx + i, pack8(g));
+    }
+    if (dbias_partial != nullptr) {
+        float4* p = reinterpret_cast<float4*>(dbias_partial + ((size_t)blockIdx.y * nvec + c) * 8);
+        p[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+        p[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+    }
+}
+
+
 }  // namespace
 
 #define BG_ALIGNED16(p) (((uintptr_t)(p) % 16) == 0)
@@ -1288,6 +1656,231 @@ extern "C" int bg_bias_tanh(const void* x, const void* bias, const void* dy, voi
     return BG_OK;
 }
 
+// ---- Swin ---------------------------------------------------------------------------------------------------------------------
+static int swin_window_args(long long mb, long long T, long long T_run, long long nW, long long L, const char* who) {
+    if (mb < 1 || nW < 1 || L < 1 || T != nW * L || T_run < T)
+        return fail(BG_EINVAL, "%s: mb %lld, windows %lld x %lld tokens and tokens %lld / %lld (run) must satisfy mb >= 1, tokens = windows "
+                    "x window tokens <= tokens_run", who, mb, nW, L, T, T_run);
+    if (T_run * mb > (1LL << 31) || L > (1 << 20)) return fail(BG_EUNSUPPORTED, "%s: too many rows", who);
+    return BG_OK;
+}
+
+extern "C" int bg_swin_window_qkv_fwd(const void* mixed, const void* bias, const int* map, void* q, void* k, void* v, long long mb,
+                                      long long tokens, long long tokens_run, long long n_windows, long long window_tokens, long long heads,
+                                      long long head_dim, void* stream) {
+    const char* who = "bg_swin_window_qkv_fwd";
+    int rc = swin_window_args(mb, tokens, tokens_run, n_windows, window_tokens, who);
+    if (rc) return rc;
+    if (heads < 1 || head_dim < 8 || head_dim % 8 || heads * head_dim * 3 / 8 > (1 << 24))
+        return fail(BG_EINVAL, "%s: heads %lld x head_dim %lld (a multiple of 8)", who, heads, head_dim);
+    if (mixed == nullptr || bias == nullptr || map == nullptr || q == nullptr || k == nullptr || v == nullptr || !BG_ALIGNED16(mixed) ||
+        !BG_ALIGNED16(bias) || !BG_ALIGNED16(q) || !BG_ALIGNED16(k) || !BG_ALIGNED16(v) || (uintptr_t)map % 4)
+        return fail(BG_EINVAL, "%s: pointers must be non-null and aligned", who);
+    const int hv = (int)(head_dim / 8);
+    const int grid = local_grid((size_t)mb * tokens * heads * 3 * hv, kThreads);
+    swin_window_qkv_fwd_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const uint4*)mixed, (const uint4*)bias, map, (uint4*)q,
+                                                                           (uint4*)k, (uint4*)v, mb, n_windows, (int)window_tokens,
+                                                                           (int)heads, hv);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_swin_window_qkv_bwd(const void* dq, const void* dk, const void* dv, void* dmixed, float* dbias_partial, int n_partial,
+                                      const int* inv, long long mb, long long tokens, long long tokens_run, long long n_windows,
+                                      long long window_tokens, long long heads, long long head_dim, void* stream) {
+    const char* who = "bg_swin_window_qkv_bwd";
+    int rc = swin_window_args(mb, tokens, tokens_run, n_windows, window_tokens, who);
+    if (rc) return rc;
+    if (heads < 1 || head_dim < 8 || head_dim % 8 || heads * head_dim * 3 / 8 > (long long)kThreads * 65535)
+        return fail(BG_EINVAL, "%s: heads %lld x head_dim %lld (a multiple of 8)", who, heads, head_dim);
+    if (n_partial < 1 || n_partial > 65535) return fail(BG_EINVAL, "%s: n_partial %d must be in [1, 65535]", who, n_partial);
+    if (dq == nullptr || dk == nullptr || dv == nullptr || dmixed == nullptr || dbias_partial == nullptr || inv == nullptr ||
+        !BG_ALIGNED16(dq) || !BG_ALIGNED16(dk) || !BG_ALIGNED16(dv) || !BG_ALIGNED16(dmixed) || !BG_ALIGNED16(dbias_partial) ||
+        (uintptr_t)inv % 4)
+        return fail(BG_EINVAL, "%s: pointers must be non-null and aligned", who);
+    const long long ncol = heads * 3 * (head_dim / 8);
+    const dim3 block = vit_block(ncol);
+    const dim3 grid((unsigned)((ncol + block.x - 1) / block.x), (unsigned)n_partial, 1);
+    swin_window_qkv_bwd_kernel<<<grid, block, 0, (cudaStream_t)stream>>>((const uint4*)dq, (const uint4*)dk, (const uint4*)dv,
+                                                                         (uint4*)dmixed, dbias_partial, inv, mb, tokens, tokens_run,
+                                                                         n_windows, (int)window_tokens, (int)heads, (int)(head_dim / 8));
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+static int swin_window_merge(const void* src, void* dst, const int* map, const int* inv, long long mb, long long tokens,
+                             long long tokens_run, long long n_windows, long long window_tokens, long long cols, bool backward,
+                             void* stream, const char* who) {
+    int rc = swin_window_args(mb, tokens, tokens_run, n_windows, window_tokens, who);
+    if (rc) return rc;
+    if (cols <= 0 || cols % 8 || cols / 8 > (1 << 24)) return fail(BG_EINVAL, "%s: cols %lld must be a positive multiple of 8", who, cols);
+    if (src == nullptr || dst == nullptr || map == nullptr || inv == nullptr || !BG_ALIGNED16(src) || !BG_ALIGNED16(dst) ||
+        (uintptr_t)map % 4 || (uintptr_t)inv % 4)
+        return fail(BG_EINVAL, "%s: pointers must be non-null and aligned", who);
+    const size_t rows = backward ? (size_t)mb * tokens : (size_t)mb * tokens_run;
+    const int grid = local_grid(rows * (cols / 8), kThreads);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (backward)
+        swin_window_merge_kernel<true><<<grid, kThreads, 0, st>>>((const uint4*)src, (uint4*)dst, map, inv, mb, tokens, tokens_run,
+                                                                  n_windows, (int)window_tokens, (int)(cols / 8));
+    else
+        swin_window_merge_kernel<false><<<grid, kThreads, 0, st>>>((const uint4*)src, (uint4*)dst, map, inv, mb, tokens, tokens_run,
+                                                                   n_windows, (int)window_tokens, (int)(cols / 8));
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_swin_window_merge_fwd(const void* windows, void* rows, const int* map, const int* inv, long long mb, long long tokens,
+                                        long long tokens_run, long long n_windows, long long window_tokens, long long cols, void* stream) {
+    return swin_window_merge(windows, rows, map, inv, mb, tokens, tokens_run, n_windows, window_tokens, cols, false, stream,
+                             "bg_swin_window_merge_fwd");
+}
+
+extern "C" int bg_swin_window_merge_bwd(const void* drows, void* dwindows, const int* map, const int* inv, long long mb, long long tokens,
+                                        long long tokens_run, long long n_windows, long long window_tokens, long long cols, void* stream) {
+    return swin_window_merge(drows, dwindows, map, inv, mb, tokens, tokens_run, n_windows, window_tokens, cols, true, stream,
+                             "bg_swin_window_merge_bwd");
+}
+
+static int merge_ln_args(long long mb, long long height, long long width, long long r, int in_bsh, long long rows_in, long long cols_in,
+                         long long tokens_out_run, MergeGeom* g, const char* who) {
+    if (r != 1 && r != 2) return fail(BG_EINVAL, "%s: merge factor %lld must be 1 or 2", who, r);
+    if (mb < 1 || height < r || width < r || height % r || width % r)
+        return fail(BG_EINVAL, "%s: a %lldx%lld token grid does not merge in %lldx%lld blocks (mb %lld)", who, height, width, r, r, mb);
+    if (cols_in <= 0 || cols_in % 8) return fail(BG_EINVAL, "%s: cols %lld must be a positive multiple of 8", who, cols_in);
+    if (r * r * cols_in / 8 > (long long)kMergeVpt * kThreads)
+        return fail(BG_EUNSUPPORTED, "%s: merged row of %lld columns > %d", who, r * r * cols_in, kMergeVpt * kThreads * 8);
+    const long long T_in = height * width, T_out = T_in / (r * r);
+    if (rows_in < mb * T_in) return fail(BG_EINVAL, "%s: rows_in %lld < mb x tokens = %lld", who, rows_in, mb * T_in);
+    if (tokens_out_run < T_out) return fail(BG_EINVAL, "%s: tokens_out_run %lld < merged tokens %lld", who, tokens_out_run, T_out);
+    if (rows_in > (1LL << 31) || tokens_out_run * mb > (1LL << 31)) return fail(BG_EUNSUPPORTED, "%s: too many rows", who);
+    g->mb = mb; g->T_in = T_in; g->T_out = T_out; g->T_out_run = tokens_out_run;
+    g->Wi = (int)width; g->Wo = (int)(width / r); g->r = (int)r; g->cvec_in = (int)(cols_in / 8); g->in_bsh = in_bsh ? 1 : 0;
+    return BG_OK;
+}
+
+extern "C" int bg_swin_merge_ln_fwd(const void* x, const void* add_bias, const void* w, const void* b, void* y, float* mean, float* rstd,
+                                    long long mb, long long height, long long width, long long r, int in_bsh, long long rows_in,
+                                    long long cols_in, long long tokens_out_run, float eps, void* stream) {
+    const char* who = "bg_swin_merge_ln_fwd";
+    MergeGeom g;
+    int rc = merge_ln_args(mb, height, width, r, in_bsh, rows_in, cols_in, tokens_out_run, &g, who);
+    if (rc) return rc;
+    if (x == nullptr || w == nullptr || b == nullptr || y == nullptr || mean == nullptr || rstd == nullptr || !BG_ALIGNED16(x) ||
+        !BG_ALIGNED16(add_bias) || !BG_ALIGNED16(w) || !BG_ALIGNED16(b) || !BG_ALIGNED16(y) || (uintptr_t)mean % 4 || (uintptr_t)rstd % 4)
+        return fail(BG_EINVAL, "%s: pointers must be non-null (add_bias may be) and aligned", who);
+    const int grid = local_grid((size_t)tokens_out_run * mb, 1);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (add_bias != nullptr)
+        swin_merge_ln_fwd_kernel<true><<<grid, kThreads, 0, st>>>((const uint4*)x, (const uint4*)add_bias, (const uint4*)w, (const uint4*)b,
+                                                                  (uint4*)y, mean, rstd, g, eps);
+    else
+        swin_merge_ln_fwd_kernel<false><<<grid, kThreads, 0, st>>>((const uint4*)x, nullptr, (const uint4*)w, (const uint4*)b, (uint4*)y,
+                                                                   mean, rstd, g, eps);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_swin_merge_ln_bwd(const void* dy, const void* x, const void* add_bias, const void* w, const float* mean, const float* rstd,
+                                    void* dx, float* dw_partial, float* db_partial, float* dbias_partial, int n_partial, long long mb,
+                                    long long height, long long width, long long r, int in_bsh, long long rows_in, long long cols_in,
+                                    void* stream) {
+    const char* who = "bg_swin_merge_ln_bwd";
+    MergeGeom g;
+    int rc = merge_ln_args(mb, height, width, r, in_bsh, rows_in, cols_in, (height / (r < 1 ? 1 : r)) * (width / (r < 1 ? 1 : r)), &g, who);
+    if (rc) return rc;
+    if (n_partial < 1 || n_partial > 65535) return fail(BG_EINVAL, "%s: n_partial %d must be in [1, 65535]", who, n_partial);
+    if ((add_bias == nullptr) != (dbias_partial == nullptr)) return fail(BG_EINVAL, "%s: add_bias and dbias_partial go together", who);
+    if (dy == nullptr || x == nullptr || w == nullptr || mean == nullptr || rstd == nullptr || dx == nullptr || dw_partial == nullptr ||
+        db_partial == nullptr || !BG_ALIGNED16(dy) || !BG_ALIGNED16(x) || !BG_ALIGNED16(add_bias) || !BG_ALIGNED16(w) ||
+        !BG_ALIGNED16(dx) || !BG_ALIGNED16(dw_partial) || !BG_ALIGNED16(db_partial) || !BG_ALIGNED16(dbias_partial) ||
+        (uintptr_t)mean % 4 || (uintptr_t)rstd % 4)
+        return fail(BG_EINVAL, "%s: pointers must be non-null (add_bias / dbias_partial may be) and aligned", who);
+    const int nvec = (int)(r * r * cols_in / 8);
+    cudaStream_t st = (cudaStream_t)stream;
+    const uint4 *dyv = (const uint4*)dy, *xv = (const uint4*)x, *bv = (const uint4*)add_bias, *wv = (const uint4*)w;
+#define BG_MERGE_BWD(V, B) swin_merge_ln_bwd_kernel<V, B><<<n_partial, kThreads, 0, st>>>(dyv, xv, bv, wv, mean, rstd, (uint4*)dx, dw_partial, db_partial, dbias_partial, g, rows_in)
+    const bool bias = add_bias != nullptr;
+    if (nvec <= kThreads) { if (bias) BG_MERGE_BWD(1, true); else BG_MERGE_BWD(1, false); }
+    else if (nvec <= 2 * kThreads) { if (bias) BG_MERGE_BWD(2, true); else BG_MERGE_BWD(2, false); }
+    else { if (bias) BG_MERGE_BWD(kMergeVpt, true); else BG_MERGE_BWD(kMergeVpt, false); }
+#undef BG_MERGE_BWD
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+static int mean_pool_args(long long tokens, long long tokens_run, long long mb, long long cols, const char* who) {
+    if (tokens < 1 || tokens_run < tokens || mb < 1) return fail(BG_EINVAL, "%s: tokens %lld / %lld (run), mb %lld", who, tokens, tokens_run, mb);
+    if (cols <= 0 || cols % 8) return fail(BG_EINVAL, "%s: cols %lld must be a positive multiple of 8", who, cols);
+    if (tokens_run * mb * (cols / 8) > (1LL << 40)) return fail(BG_EUNSUPPORTED, "%s: too large", who);
+    return BG_OK;
+}
+
+extern "C" int bg_swin_mean_pool_fwd(const void* x, void* y, long long tokens, long long tokens_run, long long mb, long long rows_out,
+                                     long long cols, void* stream) {
+    const char* who = "bg_swin_mean_pool_fwd";
+    int rc = mean_pool_args(tokens, tokens_run, mb, cols, who);
+    if (rc) return rc;
+    if (rows_out < mb) return fail(BG_EINVAL, "%s: rows_out %lld < mb %lld", who, rows_out, mb);
+    if (x == nullptr || y == nullptr || !BG_ALIGNED16(x) || !BG_ALIGNED16(y)) return fail(BG_EINVAL, "%s: pointers must be non-null and 16-B aligned", who);
+    const int grid = local_grid((size_t)rows_out * (cols / 8), kThreads);
+    swin_mean_pool_kernel<false><<<grid, kThreads, 0, (cudaStream_t)stream>>>((const uint4*)x, (uint4*)y, tokens, tokens_run, mb, rows_out,
+                                                                             (int)(cols / 8));
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_swin_mean_pool_bwd(const void* dy, void* dx, long long tokens, long long tokens_run, long long mb, long long cols,
+                                     void* stream) {
+    const char* who = "bg_swin_mean_pool_bwd";
+    int rc = mean_pool_args(tokens, tokens_run, mb, cols, who);
+    if (rc) return rc;
+    if (dy == nullptr || dx == nullptr || !BG_ALIGNED16(dy) || !BG_ALIGNED16(dx)) return fail(BG_EINVAL, "%s: pointers must be non-null and 16-B aligned", who);
+    const int grid = local_grid((size_t)tokens_run * mb * (cols / 8), kThreads);
+    swin_mean_pool_kernel<true><<<grid, kThreads, 0, (cudaStream_t)stream>>>((const uint4*)dy, (uint4*)dx, tokens, tokens_run, mb, 0,
+                                                                            (int)(cols / 8));
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_drop_path_add_fwd(const void* x, const void* bias, int bias_dtype, const void* residual, void* y, long long rows,
+                                    long long h, long long b_loc, long long sample_base, double p, unsigned seed, unsigned iteration,
+                                    unsigned site, void* stream) {
+    const char* who = "bg_drop_path_add_fwd";
+    DropoutCoords d;
+    int rc = dropout_args(rows, h, b_loc, 0, sample_base, p, seed, iteration, site, &d, who);
+    if (rc) return rc;
+    if (bias != nullptr && bias_dtype != BG_BF16 && bias_dtype != BG_F32) return fail(BG_EUNSUPPORTED, "%s: bias dtype %d", who, bias_dtype);
+    if (x == nullptr || y == nullptr || !BG_ALIGNED16(x) || !BG_ALIGNED16(bias) || !BG_ALIGNED16(residual) || !BG_ALIGNED16(y))
+        return fail(BG_EINVAL, "%s: x and y must be non-null; 16-B alignment", who);
+    if (rows == 0) return BG_OK;
+    const dim3 grid = dropout_grid(rows, h / 8, 0);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (bias != nullptr && bias_dtype == BG_F32)
+        drop_path_add_fwd_kernel<true><<<grid, kThreads, 0, st>>>((const uint4*)x, bias, (const uint4*)residual, (uint4*)y, rows, (int)(h / 8), d);
+    else
+        drop_path_add_fwd_kernel<false><<<grid, kThreads, 0, st>>>((const uint4*)x, bias, (const uint4*)residual, (uint4*)y, rows, (int)(h / 8), d);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_drop_path_add_bwd(const void* dy, void* dx, float* dbias_partial, int n_partial, long long rows, long long h,
+                                    long long b_loc, long long sample_base, double p, unsigned seed, unsigned iteration, unsigned site,
+                                    void* stream) {
+    const char* who = "bg_drop_path_add_bwd";
+    DropoutCoords d;
+    int rc = dropout_args(rows, h, b_loc, 0, sample_base, p, seed, iteration, site, &d, who);
+    if (rc) return rc;
+    if (n_partial < 1 || n_partial > 65535) return fail(BG_EINVAL, "%s: n_partial %d must be in [1, 65535]", who, n_partial);
+    if (dy == nullptr || dx == nullptr || !BG_ALIGNED16(dy) || !BG_ALIGNED16(dx) || !BG_ALIGNED16(dbias_partial))
+        return fail(BG_EINVAL, "%s: dy and dx must be non-null; 16-B alignment", who);
+    drop_path_bwd_kernel<<<dropout_grid(rows, h / 8, n_partial), kThreads, 0, (cudaStream_t)stream>>>((const uint4*)dy, (uint4*)dx,
+                                                                                                     dbias_partial, rows, (int)(h / 8), d);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+
 // loads every kernel of this file up front (see bg_preload_coll in bg_coll.cu)
 int bg_preload_ops() {
 #define K(f) reinterpret_cast<const void*>(&f)
@@ -1300,7 +1893,14 @@ int bg_preload_ops() {
                              K(dropout_add_fwd_kernel<false>), K(dropout_bwd_kernel), K(vit_patchify_kernel<true>),
                              K(vit_patchify_kernel<false>), K(vit_embed_fwd_kernel<true>), K(vit_embed_fwd_kernel<false>),
                              K(vit_embed_bwd_kernel<true>), K(vit_embed_bwd_kernel<false>), K(bias_tanh_kernel<true>),
-                             K(bias_tanh_kernel<false>)};
+                             K(bias_tanh_kernel<false>), K(swin_window_qkv_fwd_kernel), K(swin_window_qkv_bwd_kernel),
+                             K(swin_window_merge_kernel<true>), K(swin_window_merge_kernel<false>), K(swin_merge_ln_fwd_kernel<true>),
+                             K(swin_merge_ln_fwd_kernel<false>), K((swin_merge_ln_bwd_kernel<1, true>)),
+                             K((swin_merge_ln_bwd_kernel<1, false>)), K((swin_merge_ln_bwd_kernel<2, true>)),
+                             K((swin_merge_ln_bwd_kernel<2, false>)), K((swin_merge_ln_bwd_kernel<kMergeVpt, true>)),
+                             K((swin_merge_ln_bwd_kernel<kMergeVpt, false>)), K(swin_mean_pool_kernel<true>),
+                             K(swin_mean_pool_kernel<false>), K(drop_path_add_fwd_kernel<true>), K(drop_path_add_fwd_kernel<false>),
+                             K(drop_path_bwd_kernel)};
 #undef K
     for (const void* k : kernels) {
         cudaFuncAttributes attr;

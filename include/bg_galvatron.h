@@ -297,6 +297,59 @@ int bg_vit_embed_bwd(const void* dy, void* dpatch, float* dpos, float* dbias_par
  * rounding.  bias may be NULL; the dbias column sums are the caller's, as for bg_bias_gelu.  BG_EINVAL for rows < 0, cols not a
  * positive multiple of 8 or a pointer not 16-B aligned. */
 int bg_bias_tanh(const void* x, const void* bias, const void* dy, void* out, long long rows, long long cols, void* stream);
+/* Swin (swin/SwinModel_tensor_parallel.py).  Activations are SBH rows (row = token * mb + sample) of tokens_run tokens per sample,
+ * the tokens real ones first; a (possibly cyclically shifted) window partition of a layer shape is one int32 token map
+ * map[w * window_tokens + i] = the token at position i of window w, and inv its inverse (inv[map[j]] = j); window rows are
+ * [mb * n_windows][window_tokens][...], window b * n_windows + w of sample b.  tokens must equal n_windows * window_tokens; the
+ * maps must be permutations of 0..tokens-1 (the caller builds them; they are not checked).  bf16 activations, 16-B vectors.
+ * bg_swin_window_qkv_fwd: mixed [tokens_run * mb][heads * 3 * head_dim] (per head q | k | v) + bias [heads * 3 * head_dim] -> q, k, v
+ * [mb * n_windows][window_tokens][heads][head_dim], one rounding.  bg_swin_window_qkv_bwd: dmixed rows gathered from dq, dk, dv
+ * (padding-token rows zero) and dbias_partial [n_partial][heads * 3 * head_dim] fp32 per-row-group column sums in row order (the
+ * caller adds the rows; deterministic).  BG_EINVAL for inconsistent counts, head_dim not a multiple of 8, n_partial outside
+ * [1, 65535] and null or misaligned pointers. */
+int bg_swin_window_qkv_fwd(const void* mixed, const void* bias, const int* map, void* q, void* k, void* v, long long mb,
+                           long long tokens, long long tokens_run, long long n_windows, long long window_tokens, long long heads,
+                           long long head_dim, void* stream);
+int bg_swin_window_qkv_bwd(const void* dq, const void* dk, const void* dv, void* dmixed, float* dbias_partial, int n_partial,
+                           const int* inv, long long mb, long long tokens, long long tokens_run, long long n_windows,
+                           long long window_tokens, long long heads, long long head_dim, void* stream);
+/* attention output windows [mb * n_windows][window_tokens][cols] -> SBH rows [tokens_run * mb][cols] (padding-token rows zero), and
+ * the backward gather; pure copies.  BG_EINVAL as above and for cols not a positive multiple of 8. */
+int bg_swin_window_merge_fwd(const void* windows, void* rows, const int* map, const int* inv, long long mb, long long tokens,
+                             long long tokens_run, long long n_windows, long long window_tokens, long long cols, void* stream);
+int bg_swin_window_merge_bwd(const void* drows, void* dwindows, const int* map, const int* inv, long long mb, long long tokens,
+                             long long tokens_run, long long n_windows, long long window_tokens, long long cols, void* stream);
+/* Patch merging + LayerNorm.  x holds a height x width token grid of mb samples with cols_in columns: SBH rows (token * mb + b) or,
+ * with in_bsh, rows b * height * width + token (the patch GEMM's order); rows_in >= mb * height * width rows.  Output row t' * mb + b
+ * of y [tokens_out_run * mb][r * r * cols_in] (t' on the (height / r) x (width / r) grid) is the concatenation over q = 0..r*r-1 of
+ * token (r i' + (q & 1), r j' + (q >> 1)) -- HF SwinPatchMerging's x0, x1, x2, x3 -- plus add_bias (may be NULL), normalised as
+ * bg_layernorm_fwd does (same arithmetic, so the same rounding) with w, b [r * r * cols_in]; mean / rstd fp32 per output row.
+ * Padding-token rows are zero (mean = rstd = 0).  r = 1 with the patch bias is the embedding's bias + norm.  Backward: dx rows
+ * scattered to the sources (every input token feeds one output token; input rows mb * height * width .. rows_in - 1 zero) and per-CTA
+ * fp32 partials dw = sum dy * xhat, db = sum dy and, iff add_bias != NULL, dbias = sum dx.  BG_EINVAL for r not 1 or 2, a grid that
+ * does not split into r x r blocks, cols_in not a positive multiple of 8, too few rows, n_partial outside [1, 65535] and null or
+ * misaligned pointers; BG_EUNSUPPORTED for a merged row wider than 10240 columns. */
+int bg_swin_merge_ln_fwd(const void* x, const void* add_bias, const void* w, const void* b, void* y, float* mean, float* rstd,
+                         long long mb, long long height, long long width, long long r, int in_bsh, long long rows_in, long long cols_in,
+                         long long tokens_out_run, float eps, void* stream);
+int bg_swin_merge_ln_bwd(const void* dy, const void* x, const void* add_bias, const void* w, const float* mean, const float* rstd,
+                         void* dx, float* dw_partial, float* db_partial, float* dbias_partial, int n_partial, long long mb,
+                         long long height, long long width, long long r, int in_bsh, long long rows_in, long long cols_in, void* stream);
+/* Swin's pooler: x [tokens_run][mb][cols] -> y [rows_out][cols], y[b] = (fp32 sum of x[t][b] over t < tokens, in token order) /
+ * tokens, rows mb .. rows_out - 1 zero.  Backward: dx[t][b] = dy[b] / tokens for t < tokens, 0 for the padding tokens.  BG_EINVAL
+ * for tokens < 1, tokens_run < tokens, mb < 1, rows_out < mb, cols not a positive multiple of 8 and null or misaligned pointers. */
+int bg_swin_mean_pool_fwd(const void* x, void* y, long long tokens, long long tokens_run, long long mb, long long rows_out,
+                          long long cols, void* stream);
+int bg_swin_mean_pool_bwd(const void* dy, void* dx, long long tokens, long long tokens_run, long long mb, long long cols, void* stream);
+/* Per-sample drop path (stochastic depth) of Swin's attention branch on an SBH block [rows][h] whose row r is sample
+ * sample_base + r % b_loc:  y = residual + keep * scale * (x + bias), dx = keep * scale * dy with fp32 per-row-group dbias partials
+ * (as bg_dropout_bwd).  The sample is kept iff word 0 of Philox4x32-10(counter = (0, 0xffffffff, sample, iteration), key = (seed,
+ * site)) >= floor(p * 2^32); scale = 1 / (1 - p); arithmetic and argument checks as bg_dropout_add_fwd / bg_dropout_bwd (bias bf16
+ * or fp32, bias and residual may be NULL; dbias_partial may be NULL). */
+int bg_drop_path_add_fwd(const void* x, const void* bias, int bias_dtype, const void* residual, void* y, long long rows, long long h,
+                         long long b_loc, long long sample_base, double p, unsigned seed, unsigned iteration, unsigned site, void* stream);
+int bg_drop_path_add_bwd(const void* dy, void* dx, float* dbias_partial, int n_partial, long long rows, long long h, long long b_loc,
+                         long long sample_base, double p, unsigned seed, unsigned iteration, unsigned site, void* stream);
 /* host-only: one Philox4x32-10 block (the generator of curand_philox4x32_x.h), so the mask definition can be checked without a
  * GPU.  No CUDA call. */
 void bg_philox4x32_10(const uint32_t ctr[4], const uint32_t key[2], uint32_t out[4]);
