@@ -32,6 +32,34 @@ __device__ __forceinline__ float block_reduce(float v, float* smem) {
     return r;
 }
 
+// the 8 fp32 column partials of 16-B vector c in row `row` of a [rows][nvec * 8] partial array, as two float4 stores
+__device__ __forceinline__ void store_partial8(float* base, size_t row, int nvec, int c, const float acc[8]) {
+    float4* p = reinterpret_cast<float4*>(base + (row * nvec + c) * 8);
+    p[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    p[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+}
+
+// the 8 bias columns of 16-B vector c (bf16 or fp32 bias); a null bias gives zeros
+template <bool kBiasF32>
+__device__ __forceinline__ void load_bias8(const void* bias, int c, float out[8]) {
+    if (bias == nullptr) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) out[i] = 0.f;
+    } else if (kBiasF32) {
+        const float4* bp = reinterpret_cast<const float4*>(bias) + 2 * c;
+        const float4 b0 = __ldg(bp), b1 = __ldg(bp + 1);
+        out[0] = b0.x; out[1] = b0.y; out[2] = b0.z; out[3] = b0.w; out[4] = b1.x; out[5] = b1.y; out[6] = b1.z; out[7] = b1.w;
+    } else {
+        unpack8(__ldg(reinterpret_cast<const uint4*>(bias) + c), out);
+    }
+}
+
+// f[k] = keep bit k ? f[k] * scale : 0, the product rounded once (no FMA contraction with what follows)
+__device__ __forceinline__ void apply_keep8(float f[8], unsigned keep, float scale) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) f[k] = (keep >> k) & 1u ? __fmul_rn(f[k], scale) : 0.f;
+}
+
 int local_grid(size_t items, int threads) {
     long long want = (long long)((items + threads - 1) / threads);
     if (want < 1) want = 1;
@@ -207,11 +235,7 @@ __global__ void __launch_bounds__(kThreads) rmsnorm_bwd_kernel(const uint4* __re
 #pragma unroll
     for (int j = 0; j < VPT; ++j) {
         const int v = threadIdx.x + j * kThreads;
-        if (v < nvec) {
-            float4* d = reinterpret_cast<float4*>(dw_partial + ((size_t)blockIdx.x * nvec + v) * 8);
-            d[0] = make_float4(dw[j][0], dw[j][1], dw[j][2], dw[j][3]);
-            d[1] = make_float4(dw[j][4], dw[j][5], dw[j][6], dw[j][7]);
-        }
+        if (v < nvec) store_partial8(dw_partial, blockIdx.x, nvec, v, dw[j]);
     }
 }
 
@@ -326,38 +350,43 @@ __global__ void __launch_bounds__(kThreads) layernorm_bwd_kernel(const uint4* __
     for (int j = 0; j < kMaxVpt; ++j) {
         int v = threadIdx.x + j * kThreads;
         if (v < nvec) {
-            float4* d = reinterpret_cast<float4*>(dw_partial + ((size_t)blockIdx.x * nvec + v) * 8);
-            d[0] = make_float4(dw[j][0], dw[j][1], dw[j][2], dw[j][3]);
-            d[1] = make_float4(dw[j][4], dw[j][5], dw[j][6], dw[j][7]);
-            float4* e = reinterpret_cast<float4*>(db_partial + ((size_t)blockIdx.x * nvec + v) * 8);
-            e[0] = make_float4(db[j][0], db[j][1], db[j][2], db[j][3]);
-            e[1] = make_float4(db[j][4], db[j][5], db[j][6], db[j][7]);
+            store_partial8(dw_partial, blockIdx.x, nvec, v, dw[j]);
+            store_partial8(db_partial, blockIdx.x, nvec, v, db[j]);
         }
     }
 }
 
 // ---------------------------------------------------------------------------------------------
-// bias + GeLU (tanh form, Megatron's bias_gelu_impl: transformer.py:150-160 with bias_gelu_fusion; HF "gelu_new"), and the
-// exact erf form (HF BERT "gelu"):  y = gelu(x + b);  backward: dx = dy * gelu'(x + b)   (dbias = column sums of dx)
+// bias + activation:  y = act(x + b);  backward: dx = dy * act'(x + b)   (dbias = column sums of dx, the caller's)
 // ---------------------------------------------------------------------------------------------
-template <bool kTanh>
-__device__ __forceinline__ float gelu_f(float v) {
-    if (kTanh) return v * 0.5f * (1.f + tanhf(0.79788456f * v * (1.f + 0.044715f * v * v)));
-    return v * 0.5f * (1.f + erff(v * 0.70710678f));
-}
-template <bool kTanh>
-__device__ __forceinline__ float gelu_grad_f(float v) {
-    if (kTanh) {
+// GeLU, tanh form (Megatron's bias_gelu_impl: transformer.py:150-160 with bias_gelu_fusion; HF "gelu_new")
+struct GeluTanh {
+    __device__ static __forceinline__ float value(float v) { return v * 0.5f * (1.f + tanhf(0.79788456f * v * (1.f + 0.044715f * v * v))); }
+    __device__ static __forceinline__ float grad(float v) {
         const float t = tanhf(0.79788456f * v * (1.f + 0.044715f * v * v));
         return 0.5f * v * ((1.f - t * t) * (0.79788456f + 0.1070322243f * v * v)) + 0.5f * (1.f + t);
     }
-    return 0.5f * (1.f + erff(v * 0.70710678f)) + v * 0.3989422804f * __expf(-0.5f * v * v);
-}
+};
+// GeLU, exact erf form (HF BERT "gelu")
+struct GeluErf {
+    __device__ static __forceinline__ float value(float v) { return v * 0.5f * (1.f + erff(v * 0.70710678f)); }
+    __device__ static __forceinline__ float grad(float v) {
+        return 0.5f * (1.f + erff(v * 0.70710678f)) + v * 0.3989422804f * __expf(-0.5f * v * v);
+    }
+};
+// tanh (the ViT pooler: vit_hf pooler = dense + tanh)
+struct Tanh {
+    __device__ static __forceinline__ float value(float v) { return tanhf(v); }
+    __device__ static __forceinline__ float grad(float v) {
+        const float t = tanhf(v);
+        return 1.f - t * t;
+    }
+};
 
-template <bool kTanh, bool kBackward>
-__global__ void __launch_bounds__(kThreads) bias_gelu_kernel(const uint4* __restrict__ x, const uint4* __restrict__ bias,
-                                                             const uint4* __restrict__ dy, uint4* __restrict__ out,
-                                                             long long rows, int cvec) {
+template <class Act, bool kBackward>
+__global__ void __launch_bounds__(kThreads) bias_act_kernel(const uint4* __restrict__ x, const uint4* __restrict__ bias,
+                                                            const uint4* __restrict__ dy, uint4* __restrict__ out,
+                                                            long long rows, int cvec) {
     const size_t total = (size_t)rows * cvec, stride = (size_t)gridDim.x * blockDim.x;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
         const size_t c = i % cvec;
@@ -372,10 +401,10 @@ __global__ void __launch_bounds__(kThreads) bias_gelu_kernel(const uint4* __rest
             float d[8];
             unpack8(ld16_stream(dy + i), d);
 #pragma unroll
-            for (int k = 0; k < 8; ++k) f[k] = d[k] * gelu_grad_f<kTanh>(f[k]);
+            for (int k = 0; k < 8; ++k) f[k] = d[k] * Act::grad(f[k]);
         } else {
 #pragma unroll
-            for (int k = 0; k < 8; ++k) f[k] = gelu_f<kTanh>(f[k]);
+            for (int k = 0; k < 8; ++k) f[k] = Act::value(f[k]);
         }
         st16(out + i, pack8(f));
     }
@@ -409,44 +438,57 @@ __device__ __forceinline__ unsigned dropout_keep8(const DropoutCoords& d, long l
     return bits;
 }
 
+// Per-sample drop path of Swin's attention branch (stochastic depth) uses the same kernels with a per-sample mask: row r of a
+// [rows, h] SBH block is sample sample_base + r % b_loc, and the sample is kept iff word 0 of Philox4x32-10(ctr = (0, 0xffffffff,
+// sample, iteration), key = (seed, site)) >= threshold (token 0xffffffff: a counter no dropout element uses).
+__device__ __forceinline__ bool drop_path_keep(const DropoutCoords& d, long long r) {
+    const uint32_t smp = (uint32_t)(d.sample_base + r % d.b_loc);
+    return philox4x32_10(make_uint4(0u, 0xffffffffu, smp, d.iteration), make_uint2(d.seed, d.site)).x >= d.threshold;
+}
+
+// The mask policies: keep8 = the keep bits of the 8 columns starting at column 8 * c of row r.  The kernels below draw a sample
+// mask (kPerSample) before they read the row, so that a dropped sample's row is not read and a kept one keeps all 8 columns; they
+// draw an element mask after the row's loads are issued, so that the loads are in flight while Philox runs.
+struct ElementMask {
+    static constexpr bool kPerSample = false;
+    __device__ static __forceinline__ unsigned keep8(const DropoutCoords& d, long long r, int c) { return dropout_keep8(d, r, c); }
+};
+struct SampleMask {
+    static constexpr bool kPerSample = true;
+    __device__ static __forceinline__ unsigned keep8(const DropoutCoords& d, long long r, int) { return drop_path_keep(d, r) ? 0xffu : 0u; }
+};
+
 // grid = (column blocks, row groups), a thread owns one 8-column vector of every row of its group.  fp32 math in the order
 // (x + bias) * scale, then masked, then + residual, each step rounded once (__fadd_rn / __fmul_rn: no FMA contraction).
-template <bool kBiasF32>
-__global__ void __launch_bounds__(kThreads) dropout_add_fwd_kernel(const uint4* __restrict__ x, const void* __restrict__ bias,
-                                                                   const uint4* __restrict__ residual, uint4* __restrict__ y,
-                                                                   long long rows, int nvec, DropoutCoords d) {
+template <class Mask, bool kBiasF32>
+__global__ void __launch_bounds__(kThreads) bias_dropout_add_kernel(const uint4* __restrict__ x, const void* __restrict__ bias,
+                                                                    const uint4* __restrict__ residual, uint4* __restrict__ y,
+                                                                    long long rows, int nvec, DropoutCoords d) {
     const int c = blockIdx.x * kThreads + threadIdx.x;
     if (c >= nvec) return;
     float bv[8];
-    if (bias == nullptr) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) bv[i] = 0.f;
-    } else if (kBiasF32) {
-        const float4* bp = reinterpret_cast<const float4*>(bias) + 2 * c;
-        const float4 b0 = __ldg(bp), b1 = __ldg(bp + 1);
-        bv[0] = b0.x; bv[1] = b0.y; bv[2] = b0.z; bv[3] = b0.w; bv[4] = b1.x; bv[5] = b1.y; bv[6] = b1.z; bv[7] = b1.w;
-    } else {
-        unpack8(__ldg(reinterpret_cast<const uint4*>(bias) + c), bv);
-    }
+    load_bias8<kBiasF32>(bias, c, bv);
     for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
         const size_t i = (size_t)r * nvec + c;
-        const uint4 xv = ld16_stream(x + i);
-        uint4 rv = make_uint4(0u, 0u, 0u, 0u);
-        if (residual != nullptr) rv = ld16_stream(residual + i);
-        const unsigned keep = dropout_keep8(d, r, c);
         float f[8], o[8];
-        unpack8(xv, f);
-        unpack8(rv, o);
+        unpack8(residual != nullptr ? ld16_stream(residual + i) : make_uint4(0u, 0u, 0u, 0u), o);
+        if (!Mask::kPerSample || Mask::keep8(d, r, c)) {
+            unpack8(ld16_stream(x + i), f);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            const float v = (keep >> k) & 1u ? __fmul_rn(__fadd_rn(f[k], bv[k]), d.scale) : 0.f;
-            o[k] = __fadd_rn(o[k], v);
+            for (int k = 0; k < 8; ++k) f[k] = __fadd_rn(f[k], bv[k]);
+            apply_keep8(f, Mask::kPerSample ? 0xffu : Mask::keep8(d, r, c), d.scale);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) o[k] = __fadd_rn(o[k], f[k]);
+        } else {    // a dropped sample adds 0, as a dropped element does (so a -0 residual becomes +0)
+#pragma unroll
+            for (int k = 0; k < 8; ++k) o[k] = __fadd_rn(o[k], 0.f);
         }
         st16(y + i, pack8(o));
     }
 }
 
 // dx = keep * scale * dy (bf16);  dbias_partial[blockIdx.y] = the fp32 column sums of keep * scale * dy over the CTA's rows
+template <class Mask>
 __global__ void __launch_bounds__(kThreads) dropout_bwd_kernel(const uint4* __restrict__ dy, uint4* __restrict__ dx,
                                                                float* __restrict__ dbias_partial, long long rows, int nvec,
                                                                DropoutCoords d) {
@@ -457,22 +499,16 @@ __global__ void __launch_bounds__(kThreads) dropout_bwd_kernel(const uint4* __re
     for (int k = 0; k < 8; ++k) acc[k] = 0.f;
     for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
         const size_t i = (size_t)r * nvec + c;
-        const uint4 gv = ld16_stream(dy + i);
-        const unsigned keep = dropout_keep8(d, r, c);
-        float g[8];
-        unpack8(gv, g);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            g[k] = (keep >> k) & 1u ? __fmul_rn(g[k], d.scale) : 0.f;
-            acc[k] = __fadd_rn(acc[k], g[k]);
+        float g[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        if (!Mask::kPerSample || Mask::keep8(d, r, c)) {
+            unpack8(ld16_stream(dy + i), g);
+            apply_keep8(g, Mask::kPerSample ? 0xffu : Mask::keep8(d, r, c), d.scale);
         }
+#pragma unroll
+        for (int k = 0; k < 8; ++k) acc[k] = __fadd_rn(acc[k], g[k]);
         st16(dx + i, pack8(g));
     }
-    if (dbias_partial != nullptr) {
-        float4* p = reinterpret_cast<float4*>(dbias_partial + ((size_t)blockIdx.y * nvec + c) * 8);
-        p[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
-        p[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
-    }
+    if (dbias_partial != nullptr) store_partial8(dbias_partial, blockIdx.y, nvec, c, acc);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -828,11 +864,7 @@ __global__ void __launch_bounds__(kThreads) vit_embed_fwd_kernel(const uint4* __
 #pragma unroll
                 for (int k = 0; k < 8; ++k) f[k] = __fadd_rn(f[k], base[k]);
             }
-            if (kDrop) {
-                const unsigned keep = dropout_keep8(d, r, c);
-#pragma unroll
-                for (int k = 0; k < 8; ++k) f[k] = (keep >> k) & 1u ? __fmul_rn(f[k], d.scale) : 0.f;
-            }
+            if (kDrop) apply_keep8(f, dropout_keep8(d, r, c), d.scale);
             st16(y + (size_t)r * nvec + c, pack8(f));
         }
     }
@@ -860,18 +892,12 @@ __global__ void __launch_bounds__(kThreads) vit_embed_bwd_kernel(const uint4* __
             const long long r = s * b + bi;
             float g[8];
             unpack8(ld16_stream(dy + (size_t)r * nvec + c), g);
-            if (kDrop) {
-                const unsigned keep = dropout_keep8(d, r, c);
-#pragma unroll
-                for (int k = 0; k < 8; ++k) g[k] = (keep >> k) & 1u ? __fmul_rn(g[k], d.scale) : 0.f;
-            }
+            if (kDrop) apply_keep8(g, dropout_keep8(d, r, c), d.scale);
 #pragma unroll
             for (int k = 0; k < 8; ++k) acc[k] = __fadd_rn(acc[k], g[k]);
             if (s > 0) st16(dpatch + (size_t)(bi * P + s - 1) * nvec + c, pack8(g));
         }
-        float4* dp = reinterpret_cast<float4*>(dpos + ((size_t)s * nvec + c) * 8);
-        dp[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
-        dp[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+        store_partial8(dpos, s, nvec, c, acc);
         if (s > 0) {
 #pragma unroll
             for (int k = 0; k < 8; ++k) accb[k] = __fadd_rn(accb[k], acc[k]);
@@ -879,48 +905,15 @@ __global__ void __launch_bounds__(kThreads) vit_embed_bwd_kernel(const uint4* __
     }
     if (blockIdx.y == 0)
         for (long long r = b * P; r < rows_pad; ++r) st16(dpatch + (size_t)r * nvec + c, make_uint4(0u, 0u, 0u, 0u));
-    float4* p = reinterpret_cast<float4*>(dbias_partial + ((size_t)blockIdx.y * nvec + c) * 8);
-    p[0] = make_float4(accb[0], accb[1], accb[2], accb[3]);
-    p[1] = make_float4(accb[4], accb[5], accb[6], accb[7]);
-}
-
-// the ViT pooler's activation (vit_hf pooler: dense + tanh):  y = tanh(x + b);  backward: dx = dy * (1 - tanh(x + b)^2)
-template <bool kBackward>
-__global__ void __launch_bounds__(kThreads) bias_tanh_kernel(const uint4* __restrict__ x, const uint4* __restrict__ bias,
-                                                             const uint4* __restrict__ dy, uint4* __restrict__ out, long long rows,
-                                                             int cvec) {
-    const size_t total = (size_t)rows * cvec, stride = (size_t)gridDim.x * blockDim.x;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
-        const size_t c = i % cvec;
-        float f[8], b[8];
-        unpack8(ld16_stream(x + i), f);
-        if (bias != nullptr) {
-            unpack8(__ldg(bias + c), b);
-#pragma unroll
-            for (int k = 0; k < 8; ++k) f[k] += b[k];
-        }
-        if (kBackward) {
-            float g[8];
-            unpack8(ld16_stream(dy + i), g);
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                const float t = tanhf(f[k]);
-                f[k] = g[k] * (1.f - t * t);
-            }
-        } else {
-#pragma unroll
-            for (int k = 0; k < 8; ++k) f[k] = tanhf(f[k]);
-        }
-        st16(out + i, pack8(f));
-    }
+    store_partial8(dbias_partial, blockIdx.y, nvec, c, accb);
 }
 
 // ---------------------------------------------------------------------------------------------
-// Swin (swin/SwinModel_tensor_parallel.py): the window relayouts around attention, patch merging + LayerNorm, the token mean-pool
-// and the per-sample drop path.  Activations are SBH rows (row = token * mb + sample) of tokens_run tokens per sample, the real
-// tokens first; a shifted window partition is one int32 token map per layer shape: map[w * L + i] = the token at position i of
-// window w (L = window * window tokens), and inv[t] = w * L + i its inverse.  Window rows are [mb * nW, L, ...], window
-// b * nW + w of sample b.
+// Swin (swin/SwinModel_tensor_parallel.py): the window relayouts around attention, patch merging + LayerNorm and the token
+// mean-pool (its per-sample drop path is the dropout kernels' SampleMask).  Activations are SBH rows (row = token * mb + sample)
+// of tokens_run tokens per sample, the real tokens first; a shifted window partition is one int32 token map per layer shape:
+// map[w * L + i] = the token at position i of window w (L = window * window tokens), and inv[t] = w * L + i its inverse.  Window
+// rows are [mb * nW, L, ...], window b * nW + w of sample b.
 // ---------------------------------------------------------------------------------------------
 // mixed [tokens_run * mb, heads * 3 * hn] (per head q | k | v, the fused QKV GEMM's layout) + bias -> q, k, v [mb * nW, L, heads, hn]
 // (one rounding).  A thread writes one 16-B vector; consecutive threads read consecutive vectors of one mixed row.
@@ -976,9 +969,7 @@ __global__ void __launch_bounds__(kThreads) swin_window_qkv_bwd_kernel(const uin
         }
         st16(dmixed + (size_t)r * ncol + col, g);
     }
-    float4* p = reinterpret_cast<float4*>(dbias_partial + ((size_t)blockIdx.y * ncol + col) * 8);
-    p[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
-    p[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+    store_partial8(dbias_partial, blockIdx.y, ncol, col, acc);
 }
 
 // window rows [mb * nW, L, cvec vectors] <-> SBH rows [T_run * mb, cvec vectors], a pure copy.  Forward (window rows -> SBH):
@@ -1160,17 +1151,9 @@ __global__ void __launch_bounds__(kThreads) swin_merge_ln_bwd_kernel(const uint4
     for (int j = 0; j < VPT; ++j) {
         const int v = threadIdx.x + j * kThreads;
         if (v < nvec) {
-            float4* d = reinterpret_cast<float4*>(dw_partial + ((size_t)blockIdx.x * nvec + v) * 8);
-            d[0] = make_float4(dw[j][0], dw[j][1], dw[j][2], dw[j][3]);
-            d[1] = make_float4(dw[j][4], dw[j][5], dw[j][6], dw[j][7]);
-            float4* e = reinterpret_cast<float4*>(db_partial + ((size_t)blockIdx.x * nvec + v) * 8);
-            e[0] = make_float4(db[j][0], db[j][1], db[j][2], db[j][3]);
-            e[1] = make_float4(db[j][4], db[j][5], db[j][6], db[j][7]);
-            if (kBias) {
-                float4* f = reinterpret_cast<float4*>(dbias_partial + ((size_t)blockIdx.x * nvec + v) * 8);
-                f[0] = make_float4(dbi[j][0], dbi[j][1], dbi[j][2], dbi[j][3]);
-                f[1] = make_float4(dbi[j][4], dbi[j][5], dbi[j][6], dbi[j][7]);
-            }
+            store_partial8(dw_partial, blockIdx.x, nvec, v, dw[j]);
+            store_partial8(db_partial, blockIdx.x, nvec, v, db[j]);
+            if (kBias) store_partial8(dbias_partial, blockIdx.x, nvec, v, dbi[j]);
         }
     }
 }
@@ -1209,79 +1192,6 @@ __global__ void __launch_bounds__(kThreads) swin_mean_pool_kernel(const uint4* _
         st16(out + i, pack8(f));
     }
 }
-
-// Per-sample drop path of Swin's attention branch:  y = residual + keep_b * scale * (x + bias), dx = keep_b * scale * dy.  Row r
-// of a [rows, h] SBH block is sample sample_base + r % b_loc; the sample is kept iff word 0 of Philox4x32-10(ctr = (0, 0xffffffff,
-// sample, iteration), key = (seed, site)) >= threshold (token 0xffffffff: a counter no dropout element uses).  The arithmetic is
-// dropout_add_fwd_kernel's (__fadd_rn / __fmul_rn, one rounding at the end).
-__device__ __forceinline__ bool drop_path_keep(const DropoutCoords& d, long long r) {
-    const uint32_t smp = (uint32_t)(d.sample_base + r % d.b_loc);
-    return philox4x32_10(make_uint4(0u, 0xffffffffu, smp, d.iteration), make_uint2(d.seed, d.site)).x >= d.threshold;
-}
-
-template <bool kBiasF32>
-__global__ void __launch_bounds__(kThreads) drop_path_add_fwd_kernel(const uint4* __restrict__ x, const void* __restrict__ bias,
-                                                                     const uint4* __restrict__ residual, uint4* __restrict__ y,
-                                                                     long long rows, int nvec, DropoutCoords d) {
-    const int c = blockIdx.x * kThreads + threadIdx.x;
-    if (c >= nvec) return;
-    float bv[8];
-    if (bias == nullptr) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) bv[i] = 0.f;
-    } else if (kBiasF32) {
-        const float4* bp = reinterpret_cast<const float4*>(bias) + 2 * c;
-        const float4 b0 = __ldg(bp), b1 = __ldg(bp + 1);
-        bv[0] = b0.x; bv[1] = b0.y; bv[2] = b0.z; bv[3] = b0.w; bv[4] = b1.x; bv[5] = b1.y; bv[6] = b1.z; bv[7] = b1.w;
-    } else {
-        unpack8(__ldg(reinterpret_cast<const uint4*>(bias) + c), bv);
-    }
-    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
-        const size_t i = (size_t)r * nvec + c;
-        const bool keep = drop_path_keep(d, r);
-        float f[8], o[8];
-        unpack8(residual != nullptr ? ld16_stream(residual + i) : make_uint4(0u, 0u, 0u, 0u), o);
-        if (keep) {
-            unpack8(ld16_stream(x + i), f);
-#pragma unroll
-            for (int k = 0; k < 8; ++k) o[k] = __fadd_rn(o[k], __fmul_rn(__fadd_rn(f[k], bv[k]), d.scale));
-        } else {
-#pragma unroll
-            for (int k = 0; k < 8; ++k) o[k] = __fadd_rn(o[k], 0.f);
-        }
-        st16(y + i, pack8(o));
-    }
-}
-
-__global__ void __launch_bounds__(kThreads) drop_path_bwd_kernel(const uint4* __restrict__ dy, uint4* __restrict__ dx,
-                                                                 float* __restrict__ dbias_partial, long long rows, int nvec,
-                                                                 DropoutCoords d) {
-    const int c = blockIdx.x * kThreads + threadIdx.x;
-    if (c >= nvec) return;
-    float acc[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) acc[k] = 0.f;
-    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
-        const size_t i = (size_t)r * nvec + c;
-        float g[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) g[k] = 0.f;
-        if (drop_path_keep(d, r)) {
-            unpack8(ld16_stream(dy + i), g);
-#pragma unroll
-            for (int k = 0; k < 8; ++k) g[k] = __fmul_rn(g[k], d.scale);
-        }
-#pragma unroll
-        for (int k = 0; k < 8; ++k) acc[k] = __fadd_rn(acc[k], g[k]);
-        st16(dx + i, pack8(g));
-    }
-    if (dbias_partial != nullptr) {
-        float4* p = reinterpret_cast<float4*>(dbias_partial + ((size_t)blockIdx.y * nvec + c) * 8);
-        p[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
-        p[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
-    }
-}
-
 
 }  // namespace
 
@@ -1470,23 +1380,27 @@ extern "C" int bg_layernorm_bwd(const void* dy, const void* x, const void* w, co
     return BG_OK;
 }
 
-extern "C" int bg_bias_gelu(const void* x, const void* bias, const void* dy, void* out, long long rows, long long cols, int tanh_form,
-                            void* stream) {
-    if (cols <= 0 || cols % 8) return fail(BG_EINVAL, "bg_bias_gelu: cols %lld must be a positive multiple of 8", cols);
-    if (!BG_ALIGNED16(x) || !BG_ALIGNED16(bias) || !BG_ALIGNED16(dy) || !BG_ALIGNED16(out)) return fail(BG_EINVAL, "bg_bias_gelu: 16-B alignment");
-    if (rows <= 0) return BG_OK;
+// out = act(x + bias) when dy is null, else dy * act'(x + bias)
+template <class Act>
+static int bias_act(const char* who, const void* x, const void* bias, const void* dy, void* out, long long rows, long long cols,
+                    void* stream) {
+    if (cols <= 0 || cols % 8) return fail(BG_EINVAL, "%s: cols %lld must be a positive multiple of 8", who, cols);
+    if (rows < 0) return fail(BG_EINVAL, "%s: rows %lld must be >= 0", who, rows);
+    if (!BG_ALIGNED16(x) || !BG_ALIGNED16(bias) || !BG_ALIGNED16(dy) || !BG_ALIGNED16(out)) return fail(BG_EINVAL, "%s: 16-B alignment", who);
+    if (rows == 0) return BG_OK;
     const int grid = local_grid((size_t)rows * cols / 8, kThreads);
     cudaStream_t st = (cudaStream_t)stream;
     const uint4 *xv = (const uint4*)x, *bv = (const uint4*)bias, *dv = (const uint4*)dy;
-    if (dy == nullptr) {
-        if (tanh_form) bias_gelu_kernel<true, false><<<grid, kThreads, 0, st>>>(xv, bv, dv, (uint4*)out, rows, (int)(cols / 8));
-        else bias_gelu_kernel<false, false><<<grid, kThreads, 0, st>>>(xv, bv, dv, (uint4*)out, rows, (int)(cols / 8));
-    } else {
-        if (tanh_form) bias_gelu_kernel<true, true><<<grid, kThreads, 0, st>>>(xv, bv, dv, (uint4*)out, rows, (int)(cols / 8));
-        else bias_gelu_kernel<false, true><<<grid, kThreads, 0, st>>>(xv, bv, dv, (uint4*)out, rows, (int)(cols / 8));
-    }
+    if (dy == nullptr) bias_act_kernel<Act, false><<<grid, kThreads, 0, st>>>(xv, bv, dv, (uint4*)out, rows, (int)(cols / 8));
+    else bias_act_kernel<Act, true><<<grid, kThreads, 0, st>>>(xv, bv, dv, (uint4*)out, rows, (int)(cols / 8));
     BG_CHECK_LAUNCH();
     return BG_OK;
+}
+
+extern "C" int bg_bias_gelu(const void* x, const void* bias, const void* dy, void* out, long long rows, long long cols, int tanh_form,
+                            void* stream) {
+    if (tanh_form) return bias_act<GeluTanh>("bg_bias_gelu", x, bias, dy, out, rows, cols, stream);
+    return bias_act<GeluErf>("bg_bias_gelu", x, bias, dy, out, rows, cols, stream);
 }
 
 extern "C" void bg_philox4x32_10(const uint32_t ctr[4], const uint32_t key[2], uint32_t out[4]) {
@@ -1519,39 +1433,58 @@ static dim3 dropout_grid(long long rows, long long nvec, long long want_rows) {
     return dim3((unsigned)cb, (unsigned)gy, 1);
 }
 
-extern "C" int bg_dropout_add_fwd(const void* x, const void* bias, int bias_dtype, const void* residual, void* y, long long rows,
-                                  long long h, long long b_loc, long long seq_base, long long sample_base, double p, unsigned seed,
-                                  unsigned iteration, unsigned site, void* stream) {
+// y = residual + keep * scale * (x + bias) under the element (dropout) or sample (drop path) mask
+template <class Mask>
+static int bias_dropout_add(const char* who, const void* x, const void* bias, int bias_dtype, const void* residual, void* y,
+                            long long rows, long long h, long long b_loc, long long seq_base, long long sample_base, double p,
+                            unsigned seed, unsigned iteration, unsigned site, void* stream) {
     DropoutCoords d;
-    int rc = dropout_args(rows, h, b_loc, seq_base, sample_base, p, seed, iteration, site, &d, "bg_dropout_add_fwd");
+    int rc = dropout_args(rows, h, b_loc, seq_base, sample_base, p, seed, iteration, site, &d, who);
     if (rc) return rc;
-    if (bias != nullptr && bias_dtype != BG_BF16 && bias_dtype != BG_F32) return fail(BG_EUNSUPPORTED, "bg_dropout_add_fwd: bias dtype %d", bias_dtype);
-    if (!BG_ALIGNED16(x) || !BG_ALIGNED16(bias) || !BG_ALIGNED16(residual) || !BG_ALIGNED16(y))
-        return fail(BG_EINVAL, "bg_dropout_add_fwd: 16-B alignment");
+    if (bias != nullptr && bias_dtype != BG_BF16 && bias_dtype != BG_F32) return fail(BG_EUNSUPPORTED, "%s: bias dtype %d", who, bias_dtype);
+    if (x == nullptr || y == nullptr || !BG_ALIGNED16(x) || !BG_ALIGNED16(bias) || !BG_ALIGNED16(residual) || !BG_ALIGNED16(y))
+        return fail(BG_EINVAL, "%s: x and y must be non-null; 16-B alignment", who);
     if (rows == 0) return BG_OK;
     const dim3 grid = dropout_grid(rows, h / 8, 0);
     cudaStream_t st = (cudaStream_t)stream;
     if (bias != nullptr && bias_dtype == BG_F32)
-        dropout_add_fwd_kernel<true><<<grid, kThreads, 0, st>>>((const uint4*)x, bias, (const uint4*)residual, (uint4*)y, rows, (int)(h / 8), d);
+        bias_dropout_add_kernel<Mask, true><<<grid, kThreads, 0, st>>>((const uint4*)x, bias, (const uint4*)residual, (uint4*)y, rows, (int)(h / 8), d);
     else
-        dropout_add_fwd_kernel<false><<<grid, kThreads, 0, st>>>((const uint4*)x, bias, (const uint4*)residual, (uint4*)y, rows, (int)(h / 8), d);
+        bias_dropout_add_kernel<Mask, false><<<grid, kThreads, 0, st>>>((const uint4*)x, bias, (const uint4*)residual, (uint4*)y, rows, (int)(h / 8), d);
     BG_CHECK_LAUNCH();
     return BG_OK;
+}
+
+// dx = keep * scale * dy and the dbias partials, the mask regenerated from the forward's arguments
+template <class Mask>
+static int dropout_bwd(const char* who, const void* dy, void* dx, float* dbias_partial, int n_partial, long long rows, long long h,
+                       long long b_loc, long long seq_base, long long sample_base, double p, unsigned seed, unsigned iteration,
+                       unsigned site, void* stream) {
+    DropoutCoords d;
+    int rc = dropout_args(rows, h, b_loc, seq_base, sample_base, p, seed, iteration, site, &d, who);
+    if (rc) return rc;
+    if (n_partial < 1 || n_partial > 65535) return fail(BG_EINVAL, "%s: n_partial %d must be in [1, 65535]", who, n_partial);
+    if (dy == nullptr || dx == nullptr || !BG_ALIGNED16(dy) || !BG_ALIGNED16(dx) || !BG_ALIGNED16(dbias_partial))
+        return fail(BG_EINVAL, "%s: dy and dx must be non-null; 16-B alignment", who);
+    // (rows == 0 still launches: every one of the n_partial CTAs writes its partial row, zeros if it visits no row)
+    dropout_bwd_kernel<Mask><<<dropout_grid(rows, h / 8, n_partial), kThreads, 0, (cudaStream_t)stream>>>((const uint4*)dy, (uint4*)dx,
+                                                                                                         dbias_partial, rows, (int)(h / 8), d);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_dropout_add_fwd(const void* x, const void* bias, int bias_dtype, const void* residual, void* y, long long rows,
+                                  long long h, long long b_loc, long long seq_base, long long sample_base, double p, unsigned seed,
+                                  unsigned iteration, unsigned site, void* stream) {
+    return bias_dropout_add<ElementMask>("bg_dropout_add_fwd", x, bias, bias_dtype, residual, y, rows, h, b_loc, seq_base, sample_base, p,
+                                         seed, iteration, site, stream);
 }
 
 extern "C" int bg_dropout_bwd(const void* dy, void* dx, float* dbias_partial, int n_partial, long long rows, long long h, long long b_loc,
                               long long seq_base, long long sample_base, double p, unsigned seed, unsigned iteration, unsigned site,
                               void* stream) {
-    DropoutCoords d;
-    int rc = dropout_args(rows, h, b_loc, seq_base, sample_base, p, seed, iteration, site, &d, "bg_dropout_bwd");
-    if (rc) return rc;
-    if (n_partial < 1 || n_partial > 65535) return fail(BG_EINVAL, "bg_dropout_bwd: n_partial %d must be in [1, 65535]", n_partial);
-    if (!BG_ALIGNED16(dy) || !BG_ALIGNED16(dx) || !BG_ALIGNED16(dbias_partial)) return fail(BG_EINVAL, "bg_dropout_bwd: 16-B alignment");
-    // (rows == 0 still launches: every one of the n_partial CTAs writes its partial row, zeros if it visits no row)
-    dropout_bwd_kernel<<<dropout_grid(rows, h / 8, n_partial), kThreads, 0, (cudaStream_t)stream>>>((const uint4*)dy, (uint4*)dx, dbias_partial,
-                                                                                                   rows, (int)(h / 8), d);
-    BG_CHECK_LAUNCH();
-    return BG_OK;
+    return dropout_bwd<ElementMask>("bg_dropout_bwd", dy, dx, dbias_partial, n_partial, rows, h, b_loc, seq_base, sample_base, p, seed,
+                                    iteration, site, stream);
 }
 
 extern "C" int bg_vit_patchify(const void* pixels, int pixel_dtype, void* out, long long batch, long long channels, long long height,
@@ -1644,16 +1577,7 @@ extern "C" int bg_vit_embed_bwd(const void* dy, void* dpatch, float* dpos, float
 }
 
 extern "C" int bg_bias_tanh(const void* x, const void* bias, const void* dy, void* out, long long rows, long long cols, void* stream) {
-    if (cols <= 0 || cols % 8) return fail(BG_EINVAL, "bg_bias_tanh: cols %lld must be a positive multiple of 8", cols);
-    if (rows < 0) return fail(BG_EINVAL, "bg_bias_tanh: rows %lld must be >= 0", rows);
-    if (!BG_ALIGNED16(x) || !BG_ALIGNED16(bias) || !BG_ALIGNED16(dy) || !BG_ALIGNED16(out)) return fail(BG_EINVAL, "bg_bias_tanh: 16-B alignment");
-    if (rows == 0) return BG_OK;
-    const int grid = local_grid((size_t)rows * cols / 8, kThreads);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (dy == nullptr) bias_tanh_kernel<false><<<grid, kThreads, 0, st>>>((const uint4*)x, (const uint4*)bias, nullptr, (uint4*)out, rows, (int)(cols / 8));
-    else bias_tanh_kernel<true><<<grid, kThreads, 0, st>>>((const uint4*)x, (const uint4*)bias, (const uint4*)dy, (uint4*)out, rows, (int)(cols / 8));
-    BG_CHECK_LAUNCH();
-    return BG_OK;
+    return bias_act<Tanh>("bg_bias_tanh", x, bias, dy, out, rows, cols, stream);
 }
 
 // ---- Swin ---------------------------------------------------------------------------------------------------------------------
@@ -1846,61 +1770,39 @@ extern "C" int bg_swin_mean_pool_bwd(const void* dy, void* dx, long long tokens,
 extern "C" int bg_drop_path_add_fwd(const void* x, const void* bias, int bias_dtype, const void* residual, void* y, long long rows,
                                     long long h, long long b_loc, long long sample_base, double p, unsigned seed, unsigned iteration,
                                     unsigned site, void* stream) {
-    const char* who = "bg_drop_path_add_fwd";
-    DropoutCoords d;
-    int rc = dropout_args(rows, h, b_loc, 0, sample_base, p, seed, iteration, site, &d, who);
-    if (rc) return rc;
-    if (bias != nullptr && bias_dtype != BG_BF16 && bias_dtype != BG_F32) return fail(BG_EUNSUPPORTED, "%s: bias dtype %d", who, bias_dtype);
-    if (x == nullptr || y == nullptr || !BG_ALIGNED16(x) || !BG_ALIGNED16(bias) || !BG_ALIGNED16(residual) || !BG_ALIGNED16(y))
-        return fail(BG_EINVAL, "%s: x and y must be non-null; 16-B alignment", who);
-    if (rows == 0) return BG_OK;
-    const dim3 grid = dropout_grid(rows, h / 8, 0);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (bias != nullptr && bias_dtype == BG_F32)
-        drop_path_add_fwd_kernel<true><<<grid, kThreads, 0, st>>>((const uint4*)x, bias, (const uint4*)residual, (uint4*)y, rows, (int)(h / 8), d);
-    else
-        drop_path_add_fwd_kernel<false><<<grid, kThreads, 0, st>>>((const uint4*)x, bias, (const uint4*)residual, (uint4*)y, rows, (int)(h / 8), d);
-    BG_CHECK_LAUNCH();
-    return BG_OK;
+    return bias_dropout_add<SampleMask>("bg_drop_path_add_fwd", x, bias, bias_dtype, residual, y, rows, h, b_loc, 0, sample_base, p, seed,
+                                        iteration, site, stream);
 }
 
 extern "C" int bg_drop_path_add_bwd(const void* dy, void* dx, float* dbias_partial, int n_partial, long long rows, long long h,
                                     long long b_loc, long long sample_base, double p, unsigned seed, unsigned iteration, unsigned site,
                                     void* stream) {
-    const char* who = "bg_drop_path_add_bwd";
-    DropoutCoords d;
-    int rc = dropout_args(rows, h, b_loc, 0, sample_base, p, seed, iteration, site, &d, who);
-    if (rc) return rc;
-    if (n_partial < 1 || n_partial > 65535) return fail(BG_EINVAL, "%s: n_partial %d must be in [1, 65535]", who, n_partial);
-    if (dy == nullptr || dx == nullptr || !BG_ALIGNED16(dy) || !BG_ALIGNED16(dx) || !BG_ALIGNED16(dbias_partial))
-        return fail(BG_EINVAL, "%s: dy and dx must be non-null; 16-B alignment", who);
-    drop_path_bwd_kernel<<<dropout_grid(rows, h / 8, n_partial), kThreads, 0, (cudaStream_t)stream>>>((const uint4*)dy, (uint4*)dx,
-                                                                                                     dbias_partial, rows, (int)(h / 8), d);
-    BG_CHECK_LAUNCH();
-    return BG_OK;
+    return dropout_bwd<SampleMask>("bg_drop_path_add_bwd", dy, dx, dbias_partial, n_partial, rows, h, b_loc, 0, sample_base, p, seed,
+                                   iteration, site, stream);
 }
-
 
 // loads every kernel of this file up front (see bg_preload_coll in bg_coll.cu)
 int bg_preload_ops() {
 #define K(f) reinterpret_cast<const void*>(&f)
     const void* kernels[] = {K((cast_kernel<true, true>)), K((cast_kernel<true, false>)), K((cast_kernel<false, true>)), K((cast_kernel<false, false>)),
                              K(rmsnorm_fwd_kernel<1>), K(rmsnorm_fwd_kernel<2>), K(rmsnorm_fwd_kernel<4>), K(rmsnorm_bwd_kernel<1>), K(rmsnorm_bwd_kernel<2>), K(rmsnorm_bwd_kernel<4>), K(layernorm_fwd_kernel), K(layernorm_bwd_kernel),
-                             K((bias_gelu_kernel<true, false>)), K((bias_gelu_kernel<false, false>)), K((bias_gelu_kernel<true, true>)),
-                             K((bias_gelu_kernel<false, true>)), K(swiglu_fwd_kernel), K(swiglu_bwd_kernel), K(qkv_rope_kernel),
+                             K((bias_act_kernel<GeluTanh, false>)), K((bias_act_kernel<GeluErf, false>)), K((bias_act_kernel<Tanh, false>)),
+                             K((bias_act_kernel<GeluTanh, true>)), K((bias_act_kernel<GeluErf, true>)), K((bias_act_kernel<Tanh, true>)),
+                             K(swiglu_fwd_kernel), K(swiglu_bwd_kernel), K(qkv_rope_kernel),
                              K(ce_rowmax_kernel<true>), K(ce_rowmax_kernel<false>), K(ce_sumexp_kernel<true>), K(ce_sumexp_kernel<false>),
-                             K(ce_bwd_kernel<true>), K(ce_bwd_kernel<false>), K(dropout_add_fwd_kernel<true>),
-                             K(dropout_add_fwd_kernel<false>), K(dropout_bwd_kernel), K(vit_patchify_kernel<true>),
+                             K(ce_bwd_kernel<true>), K(ce_bwd_kernel<false>),
+                             K((bias_dropout_add_kernel<ElementMask, true>)), K((bias_dropout_add_kernel<ElementMask, false>)),
+                             K((bias_dropout_add_kernel<SampleMask, true>)), K((bias_dropout_add_kernel<SampleMask, false>)),
+                             K(dropout_bwd_kernel<ElementMask>), K(dropout_bwd_kernel<SampleMask>), K(vit_patchify_kernel<true>),
                              K(vit_patchify_kernel<false>), K(vit_embed_fwd_kernel<true>), K(vit_embed_fwd_kernel<false>),
-                             K(vit_embed_bwd_kernel<true>), K(vit_embed_bwd_kernel<false>), K(bias_tanh_kernel<true>),
-                             K(bias_tanh_kernel<false>), K(swin_window_qkv_fwd_kernel), K(swin_window_qkv_bwd_kernel),
+                             K(vit_embed_bwd_kernel<true>), K(vit_embed_bwd_kernel<false>),
+                             K(swin_window_qkv_fwd_kernel), K(swin_window_qkv_bwd_kernel),
                              K(swin_window_merge_kernel<true>), K(swin_window_merge_kernel<false>), K(swin_merge_ln_fwd_kernel<true>),
                              K(swin_merge_ln_fwd_kernel<false>), K((swin_merge_ln_bwd_kernel<1, true>)),
                              K((swin_merge_ln_bwd_kernel<1, false>)), K((swin_merge_ln_bwd_kernel<2, true>)),
                              K((swin_merge_ln_bwd_kernel<2, false>)), K((swin_merge_ln_bwd_kernel<kMergeVpt, true>)),
                              K((swin_merge_ln_bwd_kernel<kMergeVpt, false>)), K(swin_mean_pool_kernel<true>),
-                             K(swin_mean_pool_kernel<false>), K(drop_path_add_fwd_kernel<true>), K(drop_path_add_fwd_kernel<false>),
-                             K(drop_path_bwd_kernel)};
+                             K(swin_mean_pool_kernel<false>)};
 #undef K
     for (const void* k : kernels) {
         cudaFuncAttributes attr;

@@ -250,7 +250,7 @@ int bg_layernorm_bwd(const void* dy, const void* x, const void* w, const float* 
                      float* db_partial, long long rows, long long cols, int n_partial, void* stream);
 /* bias + GeLU of the GPT / BERT MLP (transformer.py:150-160 bias_gelu_impl): out = gelu(x + bias) when dy == NULL, else
  * out = dy * gelu'(x + bias).  tanh_form 1 = Megatron's fused / HF gelu_new, 0 = exact erf.  bias may be NULL.  BG_EINVAL for
- * cols not a positive multiple of 8 or a pointer not 16-B aligned. */
+ * rows < 0, cols not a positive multiple of 8 or a pointer not 16-B aligned. */
 int bg_bias_gelu(const void* x, const void* bias, const void* dy, void* out, long long rows, long long cols, int tanh_form, void* stream);
 /* bias + dropout + residual add of the GPT / BERT blocks, replacing the reference's F.dropout(x + bias) + residual at
  * GPTModel_tensor_parallel.py:31-39,51-59, BertModel_tensor_parallel.py:29-36,48-55 and the embedding dropouts

@@ -65,7 +65,7 @@ def test_errors_are_return_codes(bg):
     assert bg.get_tunable("comm_ctas") == 132      # one slim CTA per SM
 
 
-# Bad-argument calls of the LayerNorm and bias-GeLU entries, each with the status and message it must return.  They run in a child
+# Bad-argument calls of the LayerNorm, bias-GeLU and dropout entries, each with the status and message it must return.  They run in a child
 # process that sees no device (CUDA_VISIBLE_DEVICES=""), so a call that slips past validation fails with BG_ECUDA at its launch
 # instead of launching a kernel on a bad pointer.
 _BAD_ROW_CALLS = r"""
@@ -102,6 +102,15 @@ for i in range(4):                 # x, bias, dy, out
 call(EINVAL, GELU + ": 16-B alignment", GELU, M, None, None, A, 4, 768, 0, None)
 for cols in (0, 12):
     call(EINVAL, GELU + ": cols %d must be a positive multiple of 8" % cols, GELU, A, None, None, A, 4, cols, 1, None)
+call(EINVAL, GELU + ": rows -1 must be >= 0", GELU, A, None, None, A, -1, 768, 1, None)
+DF, DB = "bg_dropout_add_fwd", "bg_dropout_bwd"
+DROP = (8, 768, 2, 0, 0, 0.1, 1, 0, 0, None)   # rows, h, b_loc, seq_base, sample_base, p, seed, iteration, site, stream
+for i in (0, 4):                   # x, y (bias and residual may be null)
+    p = [A, None, 0, None, A]; p[i] = None
+    call(EINVAL, DF + ": x and y must be non-null; 16-B alignment", DF, *p, *DROP)
+for i in range(2):                 # dy, dx (dbias_partial may be null)
+    p = [A, A]; p[i] = None
+    call(EINVAL, DB + ": dy and dx must be non-null; 16-B alignment", DB, *p, None, 1, *DROP)
 print(json.dumps(out))
 """
 
@@ -109,12 +118,13 @@ print(json.dumps(out))
 def test_row_ops_reject_bad_arguments(bg):
     """LayerNorm and bias-GeLU validate their arguments as RMSNorm does, before any launch: BG_EINVAL for a negative row count,
     a width that is not a positive multiple of 8, a pointer that is not 16-B aligned (their 16-B vector accesses would fault)
-    and no backward partials; BG_EUNSUPPORTED for a row wider than the register-resident 8192 columns."""
+    and no backward partials; BG_EUNSUPPORTED for a row wider than the register-resident 8192 columns.  The dropout entries reject
+    a null x, y, dy or dx with BG_EINVAL, as the drop-path entries do."""
     env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
     res = subprocess.run([sys.executable, "-c", _BAD_ROW_CALLS, ROOT], env=env, capture_output=True, text=True, timeout=300)
     assert res.returncode == 0, res.stderr
     calls = json.loads(res.stdout.strip().splitlines()[-1])
-    assert len(calls) == 4 + 6 + 10 + 1 + 5 + 2
+    assert len(calls) == 4 + 6 + 10 + 1 + 5 + 2 + 1 + 2 + 2
     bad = [c for c in calls if c["got"] != c["want"]]
     assert not bad, bad
 

@@ -275,7 +275,7 @@ def _input_slack(f, v):
 
 
 def _gelu_eps(v, dy, tanh_form, rounded_input):
-    """fp32 evaluation error of the kernel's gelu (dy None) or dy * gelu' at the float64 v (see bias_gelu_kernel)."""
+    """fp32 evaluation error of the kernel's gelu (dy None) or dy * gelu' at the float64 v (see GeluTanh / GeluErf in bg_ops.cu)."""
     av = v.abs()
     if tanh_form:
         # z = c*v*(1 + a*v*v): 5 roundings and the two fp32 literals; t = tanhf(z): its 2 ulp (4 u) plus z's error through tanh'
