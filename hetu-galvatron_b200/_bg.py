@@ -96,6 +96,8 @@ SIGNATURES = {
     "bg_bias_tanh": (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _vp]),
     "bg_swin_window_qkv_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
     "bg_swin_window_qkv_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
+    "bg_cross_attn_qkv_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _vp]),
+    "bg_cross_attn_qkv_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _ll, _ll, _ll, _ll, _ll, _vp]),
     "bg_swin_window_merge_fwd": (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
     "bg_swin_window_merge_bwd": (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
     "bg_swin_merge_ln_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _i, _ll, _ll, _ll, _f, _vp]),

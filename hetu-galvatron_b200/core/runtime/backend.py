@@ -793,6 +793,31 @@ class CudaBackend:
                                                            heads, hn, _s()))
         return dmixed, dbp.sum(0)
 
+    # ---- T5 cross-attention: the query / key_value projections' outputs <-> the attention layout (include/bg_galvatron.h)
+    def cross_attn_qkv_fwd(self, q_mixed, q_bias, kv_mixed, kv_bias, heads, hn):
+        """q_mixed [s_q, b, heads * hn] + q_bias, kv_mixed [s_k, b, heads * 2 * hn] (per head k | v) + kv_bias -> q [b, s_q, heads, hn],
+        k, v [b, s_k, heads, hn]."""
+        s_q, b, s_k = q_mixed.shape[0], q_mixed.shape[1], kv_mixed.shape[0]
+        q = torch.empty(b, s_q, heads, hn, dtype=q_mixed.dtype, device=q_mixed.device)
+        k, v = [torch.empty(b, s_k, heads, hn, dtype=q_mixed.dtype, device=q_mixed.device) for _ in range(2)]
+        self.bg.check(self.bg.lib().bg_cross_attn_qkv_fwd(_p(q_mixed.contiguous()), _p(q_bias) if q_bias is not None else None,
+                                                          _p(kv_mixed.contiguous()), _p(kv_bias) if kv_bias is not None else None, _p(q),
+                                                          _p(k), _p(v), s_q, s_k, b, heads, hn, _s()))
+        return q, k, v
+
+    def cross_attn_qkv_bwd(self, dq, dk, dv):
+        """-> (dq_mixed [s_q, b, heads * hn], dkv_mixed [s_k, b, heads * 2 * hn], dq_bias, dkv_bias fp32)."""
+        b, s_q, heads, hn = dq.shape
+        s_k = dk.shape[1]
+        dqm = torch.empty(s_q, b, heads * hn, dtype=dq.dtype, device=dq.device)
+        dkvm = torch.empty(s_k, b, heads * 2 * hn, dtype=dq.dtype, device=dq.device)
+        npart = min(self.norm_partials, max(s_q, s_k) * b)
+        dbp = torch.empty(npart, heads * 3 * hn, dtype=torch.float32, device=dq.device)
+        self.bg.check(self.bg.lib().bg_cross_attn_qkv_bwd(_p(dq.contiguous()), _p(dk.contiguous()), _p(dv.contiguous()), _p(dqm), _p(dkvm),
+                                                          _p(dbp), npart, s_q, s_k, b, heads, hn, _s()))
+        db = dbp.sum(0)
+        return dqm, dkvm, db[:heads * hn], db[heads * hn:]
+
     def swin_window_merge_fwd(self, windows, tmap, inv, n_windows, mb, t_run):
         """attention output [mb * n_windows, L, heads, hn] -> SBH rows [t_run, mb, heads * hn], padding-token rows zero."""
         windows = windows.contiguous()

@@ -203,6 +203,11 @@ def _reserve_activation_staging(be, args, info, hp_whole, hp_model, tp_groups, s
     pp = hp_whole["pp_deg"]
     seq = getattr(args, "seq_length", None) or info.shapes()[0][0][0]
     hidden = getattr(args, "hidden_size", None) or info.shapes()[0][0][-1]
+    # a layer type whose boundary carries several tensors (T5's decoder: encoder output + decoder states): the relocation between two
+    # such rows moves all of them, so size for their summed sequences
+    multi = [shapes for shapes in info.shapes() if len(shapes) > 1]
+    if multi:
+        seq = max(seq, max(sum(next(d for d in s[:-1] if d != -1) for s in shapes) for shapes in multi))
     min_dp = max(1, min(hp_whole["dp_sizes_whole"]))
     max_mbs = -(-args.global_train_batch_size // min_dp // max(1, hp_model.chunks))
     esz = 2 if args.mixed_precision != "fp32" else 4

@@ -322,7 +322,9 @@ class PipelineParallel(nn.Module):
             total = 0
             for shape, dt in zip(shapes, dtypes):
                 shape = [max_microbatch_size if d == -1 else d for d in shape]
-                total += int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()
+                nb = int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()
+                # a message of several tensors starts each one on a 16-byte boundary (_StageLink.send)
+                total += nb if len(shapes) == 1 else (nb + 15) // 16 * 16
             return total
 
         if not self.is_pipeline_first_stage():

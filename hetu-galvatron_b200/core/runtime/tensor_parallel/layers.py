@@ -168,6 +168,9 @@ class LinearWithGradAccumulationAndAsyncCommunication(torch.autograd.Function):
         grad_weight = None
         if weight.requires_grad and gather_event is None:
             grad_weight = _write_wgrad(weight, dy2d, total.reshape(-1, total.shape[-1]))
+        # dgrad_addend (set by _CrossKvFn): a gradient of the input's shape that arrives from elsewhere and is summed into the dgrad --
+        # inside the GEMM epilogue when no collective follows it, else once after the collective (never once per rank)
+        addend = getattr(ctx, "dgrad_addend", None)
         if ctx.needs_input_grad[0] and not dgrad_done:
             if ctx.sequence_parallel:
                 # dgrad GEMM + reduce-scatter along the sequence (layers.py:462,488-494)
@@ -175,8 +178,13 @@ class LinearWithGradAccumulationAndAsyncCommunication(torch.autograd.Function):
                 grad_input = out.view(grad_output.shape[0] // group.size, *grad_output.shape[1:-1], k)
             elif ctx.allreduce_dgrad:
                 grad_input = be.gemm_all_reduce(dy2d, weight, "nn", group).view(*grad_output.shape[:-1], k)
+            elif addend is not None:
+                grad_input = be.gemm(dy2d, weight, "nn", addend=addend.contiguous().reshape(-1, k)).view(*grad_output.shape[:-1], k)
+                addend = None
             else:
                 grad_input = be.gemm(dy2d, weight, "nn").view(*grad_output.shape[:-1], k)
+        if addend is not None and grad_input is not None:
+            grad_input = grad_input + addend
         if gather_event is not None:
             be.wait_event(gather_event)
             grad_weight = _write_wgrad(weight, dy2d, total.reshape(-1, total.shape[-1]))

@@ -105,6 +105,45 @@ class _QkvRopeFn(torch.autograd.Function):
         return get_backend().qkv_rope_bwd(dq, dk, dv, cos, sin, ng, r, hn), None, None, None, None, None, None
 
 
+class _CrossQkvFn(torch.autograd.Function):
+    """Cross-attention relayout: the query projection's output (+ bias) and the key_value projection's output (+ bias) -> q, k, v in
+    one kernel; backward gives both projections' dgrad inputs and both biases' gradients in one kernel."""
+
+    @staticmethod
+    def forward(ctx, q_mixed, q_bias, kv_mixed, kv_bias, heads, hn):
+        ctx.bias_dtypes = (None if q_bias is None else q_bias.dtype, None if kv_bias is None else kv_bias.dtype)
+        return get_backend().cross_attn_qkv_fwd(q_mixed, q_bias, kv_mixed, kv_bias, heads, hn)
+
+    @staticmethod
+    def backward(ctx, dq, dk, dv):
+        dqm, dkvm, dqb, dkvb = get_backend().cross_attn_qkv_bwd(dq, dk, dv)
+        qdt, kvdt = ctx.bias_dtypes
+        return dqm, (None if qdt is None else dqb.to(qdt)), dkvm, (None if kvdt is None else dkvb.to(kvdt)), None, None
+
+
+class _CrossKvFn(torch.autograd.Function):
+    """The key_value projection of a cross-attention layer on the encoder output, which also returns the encoder output itself: a
+    decoder layer passes it on to the next one.  Backward sums the gradient of that pass-through into the projection's dgrad -- as the
+    dgrad GEMM's addend when no collective follows it (tensor-parallel degree 1), else once after the all-reduce / Megatron-SP
+    reduce-scatter -- instead of autograd's separate add (and buffer) per decoder layer."""
+
+    @staticmethod
+    def forward(ctx, encoder_output, weight, sequence_parallel, tp_group):
+        ctx.set_materialize_grads(False)
+        from .layers import LinearWithGradAccumulationAndAsyncCommunication as Linear
+        out = Linear.forward(ctx, encoder_output, weight, sequence_parallel, not sequence_parallel, False, tp_group)
+        return out, encoder_output
+
+    @staticmethod
+    def backward(ctx, grad_kv, grad_passthrough):
+        if grad_kv is None:
+            return grad_passthrough, None, None, None
+        from .layers import LinearWithGradAccumulationAndAsyncCommunication as Linear
+        ctx.dgrad_addend = grad_passthrough
+        grads = Linear.backward(ctx, grad_kv)
+        return grads[0], grads[1], None, None
+
+
 class _UlyssesFn(torch.autograd.Function):
     """All tensors of one exchange in one launch; backward is the inverse exchange (transformer.py:2040-2062)."""
 
@@ -461,14 +500,23 @@ class ParallelMLP(nn.Module):
 
 class ParallelAttention(nn.Module):
     """Self-attention with TP heads or Ulysses sequence parallelism, and zigzag context parallelism on its own or inside the Ulysses
-    exchange (transformer.py:512-900, :641-654)."""
+    exchange (transformer.py:512-900, :641-654).
+
+    ``AttnType.cross_attn`` (T5's decoder, transformer.py:585-620, 755-790): ``query`` on the hidden states and ``key_value`` on the
+    encoder output (per head k | v), both column-parallel, no GQA; non-causal attention of the s_q queries over the s_k keys.  Its
+    forward returns (out, bias, encoder_output): the encoder output comes back as the pass-through whose gradient the key_value
+    dgrad absorbs (``_CrossKvFn``).  Tensor parallelism and Megatron-SP only: Ulysses and context parallelism are refused."""
 
     def __init__(self, config, layer_number, attention_type=AttnType.self_attn, attn_mask_type=AttnMaskType.padding,
                  tp_group=None, sp_group=None, cp_group=None, cp_ranks=None, use_ulysses=False, use_zigzag_cp=False,
                  params_dtype=torch.float32, device=None):
         super().__init__()
-        if attention_type != AttnType.self_attn:
-            raise NotImplementedError("only self attention is on the Galvatron hot path")
+        if attention_type not in (AttnType.self_attn, AttnType.cross_attn):
+            raise NotImplementedError("attention type %r is not supported" % (attention_type,))
+        self.attention_type = attention_type
+        if attention_type == AttnType.cross_attn:
+            self._init_cross(config, layer_number, tp_group, sp_group, cp_group, use_ulysses, use_zigzag_cp, params_dtype, device)
+            return
         self.use_cp = bool(use_zigzag_cp) or _size(cp_group) > 1
         self.cp_comm = cp_comm_mode()
         self.layer_number = max(1, layer_number)
@@ -516,6 +564,51 @@ class ParallelAttention(nn.Module):
             self._rng_name = ("attention", layer_number, tp_rank, sp_rank)
             self._rng_seed = model_parallel_seed(seed, layer_number, tp_rank, sp_rank)
 
+    def _init_cross(self, config, layer_number, tp_group, sp_group, cp_group, use_ulysses, use_zigzag_cp, params_dtype, device):
+        if use_ulysses and _size(sp_group) > 1:
+            raise NotImplementedError("cross-attention under Ulysses sequence parallelism is not supported")
+        if use_zigzag_cp or _size(cp_group) > 1:
+            raise NotImplementedError("cross-attention under context parallelism is not supported")
+        n_heads = config.num_attention_heads
+        n_groups = getattr(config, "num_query_groups", None) or n_heads
+        if n_groups != n_heads:
+            raise NotImplementedError("cross-attention with grouped-query attention (num_query_groups %d != heads %d) is not supported"
+                                      % (n_groups, n_heads))
+        world = _size(tp_group)
+        assert n_heads % world == 0, "num_attention_heads must be divisible by the tensor parallel size"
+        self.use_cp, self.use_ulysses, self.cp_comm = False, False, "allgather"
+        self.layer_number = max(1, layer_number)
+        self.attn_mask_type = AttnMaskType.padding
+        self.tp_group, self.sp_group, self.cp_group = tp_group, None, None
+        self.hn = getattr(config, "kv_channels", None) or config.hidden_size // n_heads
+        self.np_local = self.ng_local = self.kv_heads_attn = n_heads // world
+        self.r = 1
+        add_bias = bool(getattr(config, "add_bias_linear", False))
+        self.query = ColumnParallelLinear(config.hidden_size, n_heads * self.hn, config=config, bias=add_bias, gather_output=False,
+                                          skip_bias_add=True, tp_group=tp_group, params_dtype=params_dtype, device=device)
+        self.key_value = ColumnParallelLinear(config.hidden_size, 2 * n_heads * self.hn, config=config, bias=add_bias, gather_output=False,
+                                              skip_bias_add=True, tp_group=tp_group, params_dtype=params_dtype, device=device)
+        self.dense = RowParallelLinear(n_heads * self.hn, config.hidden_size, config=config, bias=add_bias, skip_bias_add=True,
+                                       input_is_parallel=True, tp_group=tp_group, params_dtype=params_dtype, device=device)
+        self.softmax_scale = 1.0 / math.sqrt(self.hn)
+        self.attention_dropout = check_probability(getattr(config, "attention_dropout", 0.0), "attention_dropout")
+        if self.attention_dropout > 0.0:
+            raise NotImplementedError("attention-probability dropout in cross-attention is not supported")
+
+    def _cross_forward(self, hidden_states, encoder_output, residual):
+        """-> (out, bias, encoder_output pass-through) of cross-attention: queries from ``hidden_states`` [s_q(/t), b, h], keys and
+        values from ``encoder_output`` [s_k(/t), b, h] (Megatron-SP: both sequence-split)."""
+        if encoder_output is None:
+            raise ValueError("cross-attention needs encoder_output")
+        q_mixed, q_bias = self.query(hidden_states)                                        # [s_q, b, np * hn]
+        kv_mixed, enc_out = _CrossKvFn.apply(encoder_output, self.key_value.weight, self.key_value.sequence_parallel, self.tp_group)
+        q, k, v = _CrossQkvFn.apply(q_mixed, q_bias, kv_mixed, self.key_value.bias, self.np_local, self.hn)
+        ctxt = _attention(q, k, v, False, self.softmax_scale)                              # [b, s_q, np, hn]
+        b, s = ctxt.shape[0], ctxt.shape[1]
+        ctxt = ctxt.reshape(b, s, -1).transpose(0, 1).contiguous()
+        out, bias = self.dense(ctxt, residual=residual)
+        return out, bias, enc_out
+
     def _core_attention(self, q, k, v, causal, key_mask):
         if not (self.attention_dropout > 0.0 and self.training):
             return _attention(q, k, v, causal, self.softmax_scale, key_mask)
@@ -533,6 +626,8 @@ class ParallelAttention(nn.Module):
     def forward(self, hidden_states, attention_mask=None, encoder_output=None, inference_params=None, rotary_pos_emb=None,
                 input_recipe=None, residual=None):
         # hidden_states [sq, b, h]; rotary_pos_emb = (cos, sin) fp32 tables [sq_local, hn/2] for this rank's positions
+        if self.attention_type == AttnType.cross_attn:
+            return self._cross_forward(hidden_states, encoder_output, residual)
         mixed, _ = self.query_key_value(hidden_states, recompute=input_recipe)   # [s, b, ng*(r+2)*hn]
         cos, sin = rotary_pos_emb if rotary_pos_emb is not None else self._no_rope(mixed.shape[0], mixed.device)
         stage_group = self.sp_group if self.use_ulysses else None

@@ -1193,6 +1193,82 @@ __global__ void __launch_bounds__(kThreads) swin_mean_pool_kernel(const uint4* _
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// T5 cross-attention (t5/T5Model_tensor_parallel.py): the query and key_value projections are two GEMMs over different sequences,
+// so the fused qkv_rope relayout does not apply.  q_mixed [s_q * b, np * hn] (row = token * b + sample) + q_bias and kv_mixed
+// [s_k * b, np * 2 * hn] (per head k | v) + kv_bias -> q [b, s_q, np, hn] and k, v [b, s_k, np, hn], the bias added in fp32 and rounded
+// once (a null bias adds nothing).  One launch for both inputs: a thread writes one 16-B vector; the first s_q * b * np * hv vectors
+// are the query's, consecutive threads read consecutive vectors of one input row.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kThreads) cross_attn_qkv_fwd_kernel(const uint4* __restrict__ qm, const uint4* __restrict__ qb,
+                                                                      const uint4* __restrict__ kvm, const uint4* __restrict__ kvb,
+                                                                      uint4* __restrict__ q, uint4* __restrict__ k,
+                                                                      uint4* __restrict__ v, long long s_q, long long s_k, long long batch,
+                                                                      int heads, int hv) {
+    const int qcol = heads * hv, kvcol = 2 * qcol;
+    const size_t nq = (size_t)s_q * batch * qcol, total = nq + (size_t)s_k * batch * kvcol, stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const bool is_q = i < nq;
+        const size_t j = is_q ? i : i - nq;
+        const int ncol = is_q ? qcol : kvcol;
+        const long long r = (long long)(j / ncol);
+        const int col = (int)(j - (size_t)r * ncol);
+        const long long t = r / batch, bi = r - t * batch;
+        const uint4* bias = is_q ? qb : kvb;
+        float f[8];
+        unpack8(ld16_stream((is_q ? qm : kvm) + j), f);
+        if (bias != nullptr) {
+            float bv[8];
+            unpack8(__ldg(bias + col), bv);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) f[e] = __fadd_rn(f[e], bv[e]);
+        }
+        if (is_q) {
+            st16(q + ((size_t)bi * s_q + t) * qcol + col, pack8(f));
+        } else {
+            const int h = col / (2 * hv), part = (col / hv) & 1, e = col - (2 * h + part) * hv;
+            st16((part ? v : k) + (((size_t)bi * s_k + t) * heads + h) * hv + e, pack8(f));
+        }
+    }
+}
+
+// its backward: dq_mixed [s_q * b, np * hn] and dkv_mixed [s_k * b, np * 2 * hn] gathered from dq, dk, dv; dbias_partial[blockIdx.y]
+// [np * 3 * hn] = the CTA's fp32 column sums in row order, the query's np * hn columns first.  grid = (column blocks over both
+// outputs' columns, row groups); a thread owns one column vector of every row it visits.
+__global__ void __launch_bounds__(kThreads) cross_attn_qkv_bwd_kernel(const uint4* __restrict__ dq, const uint4* __restrict__ dk,
+                                                                      const uint4* __restrict__ dv, uint4* __restrict__ dqm,
+                                                                      uint4* __restrict__ dkvm, float* __restrict__ dbias_partial,
+                                                                      long long s_q, long long s_k, long long batch, int heads, int hv) {
+    const int qcol = heads * hv, ncol = 3 * qcol;
+    const int col = blockIdx.x * blockDim.x + threadIdx.x;
+    if (col >= ncol) return;
+    const bool is_q = col < qcol;
+    const int c = is_q ? col : col - qcol;
+    const long long s = is_q ? s_q : s_k;
+    const uint4* src = dq;
+    int off = c;
+    if (!is_q) {
+        const int h = c / (2 * hv), part = (c / hv) & 1;
+        src = part ? dv : dk;
+        off = h * hv + (c - (2 * h + part) * hv);
+    }
+    uint4* dst = is_q ? dqm : dkvm;
+    const int width = is_q ? qcol : 2 * qcol;
+    float acc[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e] = 0.f;
+    for (long long r = blockIdx.y; r < s * batch; r += gridDim.y) {
+        const long long t = r / batch, bi = r - t * batch;
+        const uint4 g = ld16_stream(src + ((size_t)bi * s + t) * qcol + off);
+        float f[8];
+        unpack8(g, f);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc[e] = __fadd_rn(acc[e], f[e]);
+        st16(dst + (size_t)r * width + c, g);
+    }
+    store_partial8(dbias_partial, blockIdx.y, ncol, col, acc);
+}
+
 }  // namespace
 
 #define BG_ALIGNED16(p) (((uintptr_t)(p) % 16) == 0)
@@ -1781,6 +1857,56 @@ extern "C" int bg_drop_path_add_bwd(const void* dy, void* dx, float* dbias_parti
                                    iteration, site, stream);
 }
 
+// ---- T5 cross-attention ---------------------------------------------------------------------------------------------------------
+static int cross_attn_args(long long s_q, long long s_k, long long batch, long long heads, long long head_dim, const char* who) {
+    if (s_q < 1 || s_k < 1 || batch < 1 || heads < 1 || head_dim < 8 || head_dim % 8)
+        return fail(BG_EINVAL, "%s: s_q %lld, s_k %lld, batch %lld, heads %lld must be >= 1 and head_dim %lld a positive multiple of 8", who,
+                    s_q, s_k, batch, heads, head_dim);
+    if (heads * 3 * (head_dim / 8) > (long long)kThreads * 65535 || (s_q > s_k ? s_q : s_k) * batch > (1LL << 40))
+        return fail(BG_EUNSUPPORTED, "%s: too many rows or columns", who);
+    return BG_OK;
+}
+
+extern "C" int bg_cross_attn_qkv_fwd(const void* q_mixed, const void* q_bias, const void* kv_mixed, const void* kv_bias, void* q, void* k,
+                                     void* v, long long s_q, long long s_k, long long batch, long long heads, long long head_dim,
+                                     void* stream) {
+    const char* who = "bg_cross_attn_qkv_fwd";
+    int rc = cross_attn_args(s_q, s_k, batch, heads, head_dim, who);
+    if (rc) return rc;
+    if (q_mixed == nullptr || kv_mixed == nullptr || q == nullptr || k == nullptr || v == nullptr || !BG_ALIGNED16(q_mixed) ||
+        !BG_ALIGNED16(q_bias) || !BG_ALIGNED16(kv_mixed) || !BG_ALIGNED16(kv_bias) || !BG_ALIGNED16(q) || !BG_ALIGNED16(k) ||
+        !BG_ALIGNED16(v))
+        return fail(BG_EINVAL, "%s: pointers must be non-null (the biases may be null) and 16-B aligned", who);
+    const int hv = (int)(head_dim / 8);
+    const int grid = local_grid((size_t)(s_q + 2 * s_k) * batch * heads * hv, kThreads);
+    cross_attn_qkv_fwd_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const uint4*)q_mixed, (const uint4*)q_bias,
+                                                                          (const uint4*)kv_mixed, (const uint4*)kv_bias, (uint4*)q,
+                                                                          (uint4*)k, (uint4*)v, s_q, s_k, batch, (int)heads, hv);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_cross_attn_qkv_bwd(const void* dq, const void* dk, const void* dv, void* dq_mixed, void* dkv_mixed, float* dbias_partial,
+                                     int n_partial, long long s_q, long long s_k, long long batch, long long heads, long long head_dim,
+                                     void* stream) {
+    const char* who = "bg_cross_attn_qkv_bwd";
+    int rc = cross_attn_args(s_q, s_k, batch, heads, head_dim, who);
+    if (rc) return rc;
+    if (n_partial < 1 || n_partial > 65535) return fail(BG_EINVAL, "%s: n_partial %d must be in [1, 65535]", who, n_partial);
+    if (dq == nullptr || dk == nullptr || dv == nullptr || dq_mixed == nullptr || dkv_mixed == nullptr || dbias_partial == nullptr ||
+        !BG_ALIGNED16(dq) || !BG_ALIGNED16(dk) || !BG_ALIGNED16(dv) || !BG_ALIGNED16(dq_mixed) || !BG_ALIGNED16(dkv_mixed) ||
+        !BG_ALIGNED16(dbias_partial))
+        return fail(BG_EINVAL, "%s: pointers must be non-null and 16-B aligned", who);
+    const long long ncol = heads * 3 * (head_dim / 8);
+    const dim3 block = vit_block(ncol);
+    const dim3 grid((unsigned)((ncol + block.x - 1) / block.x), (unsigned)n_partial, 1);
+    cross_attn_qkv_bwd_kernel<<<grid, block, 0, (cudaStream_t)stream>>>((const uint4*)dq, (const uint4*)dk, (const uint4*)dv,
+                                                                        (uint4*)dq_mixed, (uint4*)dkv_mixed, dbias_partial, s_q, s_k, batch,
+                                                                        (int)heads, (int)(head_dim / 8));
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
 // loads every kernel of this file up front (see bg_preload_coll in bg_coll.cu)
 int bg_preload_ops() {
 #define K(f) reinterpret_cast<const void*>(&f)
@@ -1802,7 +1928,7 @@ int bg_preload_ops() {
                              K((swin_merge_ln_bwd_kernel<1, false>)), K((swin_merge_ln_bwd_kernel<2, true>)),
                              K((swin_merge_ln_bwd_kernel<2, false>)), K((swin_merge_ln_bwd_kernel<kMergeVpt, true>)),
                              K((swin_merge_ln_bwd_kernel<kMergeVpt, false>)), K(swin_mean_pool_kernel<true>),
-                             K(swin_mean_pool_kernel<false>)};
+                             K(swin_mean_pool_kernel<false>), K(cross_attn_qkv_fwd_kernel), K(cross_attn_qkv_bwd_kernel)};
 #undef K
     for (const void* k : kernels) {
         cudaFuncAttributes attr;

@@ -313,6 +313,18 @@ int bg_swin_window_qkv_fwd(const void* mixed, const void* bias, const int* map, 
 int bg_swin_window_qkv_bwd(const void* dq, const void* dk, const void* dv, void* dmixed, float* dbias_partial, int n_partial,
                            const int* inv, long long mb, long long tokens, long long tokens_run, long long n_windows,
                            long long window_tokens, long long heads, long long head_dim, void* stream);
+/* T5 cross-attention (t5/T5Model_tensor_parallel.py): the two projections' outputs -> the attention library's layout.
+ * bg_cross_attn_qkv_fwd: q_mixed [s_q * batch][heads * head_dim] + q_bias and kv_mixed [s_k * batch][heads * 2 * head_dim] (per head
+ * k | v) + kv_bias, SBH rows (row = token * batch + sample) -> q [batch][s_q][heads][head_dim], k, v [batch][s_k][heads][head_dim];
+ * the bias added in fp32, one rounding; either bias may be NULL (nothing added).  bg_cross_attn_qkv_bwd: dq, dk, dv -> dq_mixed and
+ * dkv_mixed in the inputs' layouts, and dbias_partial [n_partial][heads * 3 * head_dim] fp32 per-row-group column sums in row order,
+ * the query's heads * head_dim columns first (the caller adds the rows; deterministic).  bf16, 16-B vectors; s_q * batch and
+ * s_k * batch may be odd.  BG_EINVAL for a size < 1, head_dim not a positive multiple of 8, n_partial outside [1, 65535] and null
+ * or misaligned pointers. */
+int bg_cross_attn_qkv_fwd(const void* q_mixed, const void* q_bias, const void* kv_mixed, const void* kv_bias, void* q, void* k, void* v,
+                          long long s_q, long long s_k, long long batch, long long heads, long long head_dim, void* stream);
+int bg_cross_attn_qkv_bwd(const void* dq, const void* dk, const void* dv, void* dq_mixed, void* dkv_mixed, float* dbias_partial,
+                          int n_partial, long long s_q, long long s_k, long long batch, long long heads, long long head_dim, void* stream);
 /* attention output windows [mb * n_windows][window_tokens][cols] -> SBH rows [tokens_run * mb][cols] (padding-token rows zero), and
  * the backward gather; pure copies.  BG_EINVAL as above and for cols not a positive multiple of 8. */
 int bg_swin_window_merge_fwd(const void* windows, void* rows, const int* map, const int* inv, long long mb, long long tokens,
