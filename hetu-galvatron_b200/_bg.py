@@ -90,6 +90,8 @@ SIGNATURES = {
     "bg_bias_gelu": (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _i, _vp]),
     "bg_dropout_add_fwd": (_i, [_vp, _vp, _i, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _c.c_double, _c.c_uint, _c.c_uint, _c.c_uint, _vp]),
     "bg_dropout_bwd": (_i, [_vp, _vp, _vp, _i, _ll, _ll, _ll, _ll, _ll, _c.c_double, _c.c_uint, _c.c_uint, _c.c_uint, _vp]),
+    "bg_dropout_add_fwd_ids": (_i, [_vp, _vp, _i, _vp, _vp, _ll, _ll, _ll, _ll, _vp, _c.c_double, _c.c_uint, _c.c_uint, _c.c_uint, _vp]),
+    "bg_dropout_bwd_ids": (_i, [_vp, _vp, _vp, _i, _ll, _ll, _ll, _ll, _vp, _c.c_double, _c.c_uint, _c.c_uint, _c.c_uint, _vp]),
     "bg_vit_patchify": (_i, [_vp, _i, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
     "bg_vit_embed_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _c.c_double, _c.c_uint, _c.c_uint, _c.c_uint, _vp]),
     "bg_vit_embed_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _ll, _ll, _ll, _ll, _ll, _ll, _c.c_double, _c.c_uint, _c.c_uint, _c.c_uint, _vp]),

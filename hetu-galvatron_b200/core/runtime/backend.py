@@ -925,6 +925,41 @@ class CudaBackend:
                                                    _s()))
         return dx, (dbp.sum(0) if dbp is not None else None)
 
+    @staticmethod
+    def _check_sample_ids(ids, b, x):
+        assert ids.dtype == torch.int32 and ids.shape == (b,) and ids.is_contiguous() and ids.device == x.device, \
+            "sample_ids must be a contiguous int32 [%d] tensor on %s" % (b, x.device)
+
+    def dropout_add_fwd_ids(self, x, bias, residual, p, seed, iteration, site, seq_base, sample_ids):
+        """``dropout_add_fwd`` with row r of x [s_loc, b_loc, h] at sample ``sample_ids[r % b_loc]`` (int32 [b_loc] on x's device, read
+        as uint32): the samples a relocation gathered from several data-parallel ranks."""
+        s, b, h = x.shape
+        self._check_sample_ids(sample_ids, b, x)
+        x = x.contiguous()
+        y = torch.empty_like(x)
+        if residual is not None:
+            residual = residual.contiguous()
+            assert residual.shape == x.shape and residual.dtype == x.dtype
+        bcode = self.bg.dtype_code(bias.dtype) if bias is not None else 0
+        self.bg.check(self.bg.lib().bg_dropout_add_fwd_ids(_p(x), _p(bias) if bias is not None else None, bcode,
+                                                           _p(residual) if residual is not None else None, _p(y), s * b, h, b,
+                                                           int(seq_base), _p(sample_ids), float(p), int(seed), int(iteration),
+                                                           int(site), _s()))
+        return y
+
+    def dropout_bwd_ids(self, dy, p, seed, iteration, site, seq_base, sample_ids, with_bias):
+        """``dropout_bwd`` at the sample map of ``dropout_add_fwd_ids``."""
+        s, b, h = dy.shape
+        self._check_sample_ids(sample_ids, b, dy)
+        dy = dy.contiguous()
+        dx = torch.empty_like(dy)
+        npart = min(self.norm_partials, max(1, s * b))
+        dbp = torch.empty(npart, h, dtype=torch.float32, device=dy.device) if with_bias else None
+        self.bg.check(self.bg.lib().bg_dropout_bwd_ids(_p(dy), _p(dx), _p(dbp) if dbp is not None else None, npart, s * b, h, b,
+                                                       int(seq_base), _p(sample_ids), float(p), int(seed), int(iteration), int(site),
+                                                       _s()))
+        return dx, (dbp.sum(0) if dbp is not None else None)
+
     def swiglu_fwd(self, gate_up):
         rows, two_f = gate_up.reshape(-1, gate_up.shape[-1]).shape
         y = torch.empty(gate_up.shape[:-1] + (two_f // 2,), dtype=gate_up.dtype, device=gate_up.device)

@@ -18,6 +18,7 @@ from .comm_groups import gen_comm_groups
 from .hybrid_parallel_config import (check_hp_config, get_chunks, hp_config_whole_model, layer_shapes_dtypes_whole_model,
                                      mixed_precision_dtype)
 from .parallel import finalize_pools, wrap_modules_relocation
+from .sample_layout import derive_sample_layouts
 from .tensor_parallel import random as dropout_random
 from .tensor_parallel.transformer import ParallelAttention, cp_comm_mode
 
@@ -40,11 +41,12 @@ class GalvatronModel(nn.Module):
             loss_func = self.fake_loss_func
             assert isinstance(batch, (tuple, list))
             batch = [batch, [self.fake_tensor(batch[0])]]
-        # dropout coordinates of this step: the iteration, and the global index of this rank's first sample (the batch is split
-        # contiguously over the data-parallel ranks of the vocabulary rows)
+        # dropout coordinates of this step: the iteration, the global index of this rank's first sample (the batch is split
+        # contiguously over the data-parallel ranks of the vocabulary rows), and which of the samples each row holds
         dp = getattr(self, "vtp_data_group", None)
         local = next((t.shape[0] for t in batch[0] if torch.is_tensor(t)), 0)
-        dropout_random.begin_iteration(getattr(args, "seed", 0), self.iter, (dp.rank_in_group() if dp is not None else 0) * local)
+        dropout_random.begin_iteration(getattr(args, "seed", 0), self.iter, (dp.rank_in_group() if dp is not None else 0) * local,
+                                       getattr(self, "sample_layouts", None), local)
         if args.pp_deg > 1:
             if args.pipeline_type == "gpipe":
                 loss = model.gpipe_forward(batch, loss_func, **kwargs)
@@ -134,6 +136,9 @@ def construct_hybrid_parallel_model_api(model, model_config, training_args, hybr
         raise ValueError("this strategy changes the context-parallel degree between rows: it needs --sequence-parallel "
                          "(the relocation re-splits the sequence only under that flag, redistribute.py:60,121)")
 
+    # which samples each of this rank's rows holds once the relocations have split / gathered the batch (dropout draws there)
+    sample_layouts = derive_sample_layouts(hp_whole, _world.get_rank(), _world.get_world_size())
+
     # [Step 0] communication groups (pure rank lists)
     (pp_group, tp_groups_whole, sp_groups_whole, cp_groups_whole, dp_groups_whole, seq_data_groups_whole,
      allgather_tp_sp_groups_whole, split_tp_sp_groups_whole, allgather_cp_groups_whole, split_cp_groups_whole,
@@ -192,6 +197,7 @@ def construct_hybrid_parallel_model_api(model, model_config, training_args, hybr
     gm.cp_groups_whole, gm.sdp_groups_whole = cp_groups_whole, seq_data_groups_whole
     gm.hybrid_parallel_configs, gm.vtp_data_group = hybrid_parallel_configs, vtp_data_group
     gm.pp_group, gm.embedding_group, gm.hp_configs_whole = pp_group, embedding_group, hp_whole
+    gm.sample_layouts = sample_layouts
     return gm
 
 

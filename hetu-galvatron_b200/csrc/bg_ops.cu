@@ -2,6 +2,7 @@
 // (SURVEY 2.3 rows K5 RMSNorm, K6 swiglu, K9 RoPE + the split/transposes of transformer.py:731-867,
 //  a10 vocab-parallel cross-entropy).  All HBM-bound: 16-B vector access, fp32 math, one rounding to bf16.
 #include "bg_common.cuh"
+#include <type_traits>
 
 using namespace bg;
 
@@ -419,7 +420,11 @@ __global__ void __launch_bounds__(kThreads) bias_act_kernel(const uint4* __restr
 // and backward regenerates it (nothing stored).
 // ---------------------------------------------------------------------------------------------
 struct DropoutCoords {
-    long long b_loc, seq_base, sample_base;
+    long long b_loc, seq_base;
+    union {
+        long long sample_base;          // row r is sample sample_base + r % b_loc
+        const uint32_t* sample_ids;     // IdMask: row r is sample sample_ids[r % b_loc]
+    };
     uint32_t threshold, seed, iteration, site;
     float scale;
 };
@@ -428,6 +433,22 @@ struct DropoutCoords {
 __device__ __forceinline__ unsigned dropout_keep8(const DropoutCoords& d, long long r, int c) {
     const long long tok = r / d.b_loc;
     const uint32_t t = (uint32_t)(d.seq_base + tok), smp = (uint32_t)(d.sample_base + (r - tok * d.b_loc));
+    const uint2 key = make_uint2(d.seed, d.site);
+    const uint4 a = philox4x32_10(make_uint4(2u * c, t, smp, d.iteration), key);
+    const uint4 b = philox4x32_10(make_uint4(2u * c + 1u, t, smp, d.iteration), key);
+    const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    unsigned bits = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) bits |= (w[i] >= d.threshold ? 1u : 0u) << i;
+    return bits;
+}
+
+// the same bits with row r's sample read from the map: sample_ids[r % b_loc].  (A shared helper taking (t, sample) would be one
+// definition, but it changes the register allocation of every kernel that inlines dropout_keep8; the Philox counter, key and
+// threshold here are dropout_keep8's, term for term.)
+__device__ __forceinline__ unsigned dropout_keep8_ids(const DropoutCoords& d, long long r, int c) {
+    const long long tok = r / d.b_loc;
+    const uint32_t t = (uint32_t)(d.seq_base + tok), smp = __ldg(d.sample_ids + (r - tok * d.b_loc));
     const uint2 key = make_uint2(d.seed, d.site);
     const uint4 a = philox4x32_10(make_uint4(2u * c, t, smp, d.iteration), key);
     const uint4 b = philox4x32_10(make_uint4(2u * c + 1u, t, smp, d.iteration), key);
@@ -456,6 +477,12 @@ struct ElementMask {
 struct SampleMask {
     static constexpr bool kPerSample = true;
     __device__ static __forceinline__ unsigned keep8(const DropoutCoords& d, long long r, int) { return drop_path_keep(d, r) ? 0xffu : 0u; }
+};
+// the element mask at an explicit sample map: row r is sample sample_ids[r % b_loc] (the samples a layer holds after a relocation
+// re-split the batch are not one run of consecutive indices); counter, key, threshold and scale as ElementMask
+struct IdMask {
+    static constexpr bool kPerSample = false;
+    __device__ static __forceinline__ unsigned keep8(const DropoutCoords& d, long long r, int c) { return dropout_keep8_ids(d, r, c); }
 };
 
 // grid = (column blocks, row groups), a thread owns one 8-column vector of every row of its group.  fp32 math in the order
@@ -1509,13 +1536,24 @@ static dim3 dropout_grid(long long rows, long long nvec, long long want_rows) {
     return dim3((unsigned)cb, (unsigned)gy, 1);
 }
 
-// y = residual + keep * scale * (x + bias) under the element (dropout) or sample (drop path) mask
+// the sample map of an IdMask launch: BG_EINVAL for a null or not 4-B aligned one (its entries are read as 32-bit words)
+template <class Mask>
+static int sample_ids_arg(const uint32_t* sample_ids, DropoutCoords* d, const char* who) {
+    if (!std::is_same<Mask, IdMask>::value) return BG_OK;
+    if (sample_ids == nullptr || reinterpret_cast<uintptr_t>(sample_ids) % 4)
+        return fail(BG_EINVAL, "%s: sample_ids must be non-null and 4-B aligned", who);
+    d->sample_ids = sample_ids;
+    return BG_OK;
+}
+
+// y = residual + keep * scale * (x + bias) under the element (dropout), element-at-a-sample-map or sample (drop path) mask
 template <class Mask>
 static int bias_dropout_add(const char* who, const void* x, const void* bias, int bias_dtype, const void* residual, void* y,
                             long long rows, long long h, long long b_loc, long long seq_base, long long sample_base, double p,
-                            unsigned seed, unsigned iteration, unsigned site, void* stream) {
+                            unsigned seed, unsigned iteration, unsigned site, void* stream, const uint32_t* sample_ids = nullptr) {
     DropoutCoords d;
     int rc = dropout_args(rows, h, b_loc, seq_base, sample_base, p, seed, iteration, site, &d, who);
+    if (!rc) rc = sample_ids_arg<Mask>(sample_ids, &d, who);
     if (rc) return rc;
     if (bias != nullptr && bias_dtype != BG_BF16 && bias_dtype != BG_F32) return fail(BG_EUNSUPPORTED, "%s: bias dtype %d", who, bias_dtype);
     if (x == nullptr || y == nullptr || !BG_ALIGNED16(x) || !BG_ALIGNED16(bias) || !BG_ALIGNED16(residual) || !BG_ALIGNED16(y))
@@ -1535,9 +1573,10 @@ static int bias_dropout_add(const char* who, const void* x, const void* bias, in
 template <class Mask>
 static int dropout_bwd(const char* who, const void* dy, void* dx, float* dbias_partial, int n_partial, long long rows, long long h,
                        long long b_loc, long long seq_base, long long sample_base, double p, unsigned seed, unsigned iteration,
-                       unsigned site, void* stream) {
+                       unsigned site, void* stream, const uint32_t* sample_ids = nullptr) {
     DropoutCoords d;
     int rc = dropout_args(rows, h, b_loc, seq_base, sample_base, p, seed, iteration, site, &d, who);
+    if (!rc) rc = sample_ids_arg<Mask>(sample_ids, &d, who);
     if (rc) return rc;
     if (n_partial < 1 || n_partial > 65535) return fail(BG_EINVAL, "%s: n_partial %d must be in [1, 65535]", who, n_partial);
     if (dy == nullptr || dx == nullptr || !BG_ALIGNED16(dy) || !BG_ALIGNED16(dx) || !BG_ALIGNED16(dbias_partial))
@@ -1561,6 +1600,20 @@ extern "C" int bg_dropout_bwd(const void* dy, void* dx, float* dbias_partial, in
                               void* stream) {
     return dropout_bwd<ElementMask>("bg_dropout_bwd", dy, dx, dbias_partial, n_partial, rows, h, b_loc, seq_base, sample_base, p, seed,
                                     iteration, site, stream);
+}
+
+extern "C" int bg_dropout_add_fwd_ids(const void* x, const void* bias, int bias_dtype, const void* residual, void* y, long long rows,
+                                      long long h, long long b_loc, long long seq_base, const uint32_t* sample_ids, double p, unsigned seed,
+                                      unsigned iteration, unsigned site, void* stream) {
+    return bias_dropout_add<IdMask>("bg_dropout_add_fwd_ids", x, bias, bias_dtype, residual, y, rows, h, b_loc, seq_base, 0, p, seed,
+                                    iteration, site, stream, sample_ids);
+}
+
+extern "C" int bg_dropout_bwd_ids(const void* dy, void* dx, float* dbias_partial, int n_partial, long long rows, long long h,
+                                  long long b_loc, long long seq_base, const uint32_t* sample_ids, double p, unsigned seed,
+                                  unsigned iteration, unsigned site, void* stream) {
+    return dropout_bwd<IdMask>("bg_dropout_bwd_ids", dy, dx, dbias_partial, n_partial, rows, h, b_loc, seq_base, 0, p, seed, iteration,
+                               site, stream, sample_ids);
 }
 
 extern "C" int bg_vit_patchify(const void* pixels, int pixel_dtype, void* out, long long batch, long long channels, long long height,
@@ -1919,7 +1972,9 @@ int bg_preload_ops() {
                              K(ce_bwd_kernel<true>), K(ce_bwd_kernel<false>),
                              K((bias_dropout_add_kernel<ElementMask, true>)), K((bias_dropout_add_kernel<ElementMask, false>)),
                              K((bias_dropout_add_kernel<SampleMask, true>)), K((bias_dropout_add_kernel<SampleMask, false>)),
-                             K(dropout_bwd_kernel<ElementMask>), K(dropout_bwd_kernel<SampleMask>), K(vit_patchify_kernel<true>),
+                             K(dropout_bwd_kernel<ElementMask>), K(dropout_bwd_kernel<SampleMask>),
+                             K((bias_dropout_add_kernel<IdMask, true>)), K((bias_dropout_add_kernel<IdMask, false>)),
+                             K(dropout_bwd_kernel<IdMask>), K(vit_patchify_kernel<true>),
                              K(vit_patchify_kernel<false>), K(vit_embed_fwd_kernel<true>), K(vit_embed_fwd_kernel<false>),
                              K(vit_embed_bwd_kernel<true>), K(vit_embed_bwd_kernel<false>),
                              K(swin_window_qkv_fwd_kernel), K(swin_window_qkv_bwd_kernel),

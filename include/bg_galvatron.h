@@ -268,6 +268,16 @@ int bg_dropout_add_fwd(const void* x, const void* bias, int bias_dtype, const vo
 int bg_dropout_bwd(const void* dy, void* dx, float* dbias_partial, int n_partial, long long rows, long long h, long long b_loc,
                    long long seq_base, long long sample_base, double p, unsigned seed, unsigned iteration, unsigned site,
                    void* stream);
+/* the same pair at an explicit sample map: row r is sample sample_ids[r % b_loc] (device memory, b_loc uint32 entries) instead of
+ * sample_base + r % b_loc; the mask, arithmetic and every other argument as bg_dropout_add_fwd / bg_dropout_bwd.  For the layers
+ * whose samples a relocation gathered from several data-parallel ranks' microbatches: not one run of consecutive indices.
+ * BG_EINVAL as those entries, and for a null or not 4-B aligned sample_ids. */
+int bg_dropout_add_fwd_ids(const void* x, const void* bias, int bias_dtype, const void* residual, void* y, long long rows, long long h,
+                           long long b_loc, long long seq_base, const uint32_t* sample_ids, double p, unsigned seed, unsigned iteration,
+                           unsigned site, void* stream);
+int bg_dropout_bwd_ids(const void* dy, void* dx, float* dbias_partial, int n_partial, long long rows, long long h, long long b_loc,
+                       long long seq_base, const uint32_t* sample_ids, double p, unsigned seed, unsigned iteration, unsigned site,
+                       void* stream);
 /* ViT front end (vit_hf/ViTModel_sequential.py ViTEmbeddings_).  bg_vit_patchify: pixels [batch][channels][height][width] (BG_BF16
  * or BG_F32) -> bf16 patch rows out [rows_pad][patch * patch * channels] in einops' "b c (h p1) (w p2) -> b (h w) (p1 p2 c)" order
  * (fp32 pixels rounded once, RNE); rows batch * P .. rows_pad - 1 are zeros, P = (height / patch) * (width / patch).
