@@ -930,10 +930,20 @@ extern "C" int bg_reduce_scatter_acc(bg_ctx_t c, int gid, int lane, const size_t
                                  postscale, stream);
 }
 
+// The checks of the three AdamW entries, before any launch.  The hyperparameters are checked as the fp32 values the kernels use
+// (torch.optim.AdamW's constructor checks, in fp32): beta1 = 1 would make bias_corr1 0 and every parameter inf or NaN.
 static int adam_out(float* param, float* exp_avg, float* exp_avg_sq, float lr, float beta1, float beta2, float eps,
                     float weight_decay, long long step, RsOut* o) {
+    if (param == nullptr || exp_avg == nullptr || exp_avg_sq == nullptr)
+        return fail(BG_EINVAL, "adamw: param, exp_avg and exp_avg_sq must be non-null");
     if (((uintptr_t)param | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) % 16) return fail(BG_EINVAL, "optimizer state not 16-B aligned");
     if (step < 1) return fail(BG_EINVAL, "adam step must be >= 1");
+    if (!(lr >= 0.f && isfinite(lr))) return fail(BG_EINVAL, "adamw: lr %g must be finite and >= 0", lr);
+    if (!(eps >= 0.f && isfinite(eps))) return fail(BG_EINVAL, "adamw: eps %g must be finite and >= 0", eps);
+    if (!(weight_decay >= 0.f && isfinite(weight_decay)))
+        return fail(BG_EINVAL, "adamw: weight_decay %g must be finite and >= 0", weight_decay);
+    if (!(beta1 >= 0.f && beta1 < 1.f)) return fail(BG_EINVAL, "adamw: beta1 %g outside [0, 1)", beta1);
+    if (!(beta2 >= 0.f && beta2 < 1.f)) return fail(BG_EINVAL, "adamw: beta2 %g outside [0, 1)", beta2);
     o->dst = param; o->exp_avg = exp_avg; o->exp_avg_sq = exp_avg_sq;
     o->a.lr = lr; o->a.beta1 = beta1; o->a.beta2 = beta2; o->a.eps = eps; o->a.weight_decay = weight_decay;
     o->a.bias_corr1 = (float)(1.0 - pow((double)beta1, (double)step));
@@ -972,6 +982,8 @@ extern "C" int bg_reduce_scatter_sumsq(bg_ctx_t c, int gid, int lane, const size
     for (int r = 0; r < n_skip; ++r) {
         if (skip[2 * r] % 8 || skip[2 * r + 1] % 8 || skip[2 * r] > skip[2 * r + 1])
             return fail(BG_EINVAL, "skip range [%zu, %zu) is not 8-element aligned", skip[2 * r], skip[2 * r + 1]);
+        if (skip[2 * r + 1] > shard_elems)
+            return fail(BG_EINVAL, "skip range [%zu, %zu) ends past the shard of %zu elements", skip[2 * r], skip[2 * r + 1], shard_elems);
         o.skip_lo[r] = skip[2 * r]; o.skip_hi[r] = skip[2 * r + 1];
     }
     if (dst != nullptr && (uintptr_t)dst % 16) return fail(BG_EINVAL, "dst not 16-B aligned");
@@ -984,6 +996,7 @@ extern "C" int bg_adamw_clipped(float* param, float* exp_avg, float* exp_avg_sq,
     int rc = adam_out(param, exp_avg, exp_avg_sq, lr, beta1, beta2, eps, weight_decay, step, &o);
     if (rc) return rc;
     if (n % 4 || (uintptr_t)grad % 16) return fail(BG_EINVAL, "adamw: %zu elements / gradient alignment (need multiples of 4, 16 B)", n);
+    if (n > 0 && grad == nullptr) return fail(BG_EINVAL, "adamw: null grad");
     if (n == 0) return BG_OK;
     o.clip_coef = clip_coef;
     const int grid = comm_grid(n / 4, kThreads, 1);

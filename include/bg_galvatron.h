@@ -131,7 +131,18 @@ int bg_reduce_scatter_acc(bg_ctx_t ctx, int gid, int lane, const size_t* src_off
 
 /* C2 + optimizer (SURVEY 8f-3): the same pull reduce-scatter, but the reduced gradient is consumed in registers by an AdamW
  * step on the caller's fp32 shard (param, exp_avg, exp_avg_sq) -- the fp32 gradient shard is never written.  Update rule of
- * torch.optim.AdamW / apex FusedAdam adam_w_mode (galvatron/core/runtime/utils.py:137-150); `step` >= 1 for bias correction. */
+ * torch.optim.AdamW / apex FusedAdam adam_w_mode (galvatron/core/runtime/utils.py:137-150); `step` >= 1 for bias correction.
+ * In fp32, per element, with g = (sum prescale * x) * postscale rounded once (bit for bit bg_reduce_scatter_acc's fp32 output):
+ *   m = beta1 * m + (1 - beta1) * g;  v = beta2 * v + (1 - beta2) * g * g
+ *   p = p * (1 - lr * weight_decay) - (lr / bias_corr1) * m / (sqrt(v) / bias_corr2_sqrt + eps)
+ * (multiply-adds may be contracted).  The hyperparameters are the fp32 values received here, not the caller's doubles: 1 - beta
+ * is formed in fp32 from the fp32 beta (at beta2 = 0.999, 1 - 0.999f is 1.3e-5 relative away from 1 - 0.999), and
+ * bias_corr1 = 1 - beta1^step and bias_corr2_sqrt = sqrt(1 - beta2^step) are computed in double from the fp32 betas and then
+ * rounded to fp32.
+ * Errors of the three AdamW entries (this one, _clipped and bg_adamw_clipped), in this order, before the context is looked at and
+ * before any launch, all BG_EINVAL: a null param, exp_avg or exp_avg_sq; any of them not 16-B aligned; step < 1; lr, eps or
+ * weight_decay negative or not finite; beta1 or beta2 outside [0, 1) or NaN (torch.optim.AdamW's checks, on the fp32 values).
+ * Then the errors of bg_reduce_scatter_acc with an fp32 dst. */
 int bg_reduce_scatter_adamw(bg_ctx_t ctx, int gid, int lane, const size_t* src_offs, int src_dtype, float* param, float* exp_avg,
                             float* exp_avg_sq, size_t shard_elems, float prescale, float postscale, float lr, float beta1,
                             float beta2, float eps, float weight_decay, long long step, void* stream);
@@ -142,21 +153,29 @@ int bg_reduce_scatter_adamw(bg_ctx_t ctx, int gid, int lane, const size_t* src_o
  * when `n_partials` is too small -- 4 x comm_ctas, or 4 x local_ctas for a group of one, always suffice).  The sums accumulate in
  * fp64 in a fixed order: no atomics, run-to-run deterministic.  `skip` holds `n_skip` (<= BG_MAX_SKIP) shard-relative element
  * ranges [lo, hi), multiples of 8, left out of the sum (tensor-parallel duplicates).  `dst` null: nothing else is written; non-null:
- * also the fp32 shard, bit-identical to bg_reduce_scatter_acc's (accumulate 0). */
+ * also the fp32 shard, bit-identical to bg_reduce_scatter_acc's (accumulate 0).  Ranges may touch or overlap (an element in
+ * several ranges is left out once); a range with lo = hi is empty.
+ * Errors, BG_EINVAL, in this order and before any launch: null `partials` or n_partials < 1; n_skip outside [0, BG_MAX_SKIP]; a
+ * range whose bounds are not multiples of 8 or with lo > hi; a range with hi > shard_elems; dst not 16-B aligned; then those of
+ * bg_reduce_scatter_acc, then a launch that needs more than n_partials entries. */
 #define BG_MAX_SKIP 16
 int bg_reduce_scatter_sumsq(bg_ctx_t ctx, int gid, int lane, const size_t* src_offs, int src_dtype, float* dst, size_t shard_elems,
                             float prescale, float postscale, float* partials, int n_partials, const size_t* skip, int n_skip,
                             void* stream);
 
 /* Step pass: bg_reduce_scatter_adamw with the reduced gradient multiplied by the device scalar *clip_coef (null: 1) before the
- * moments are updated.  At a coefficient of 1 the result is bit-identical to bg_reduce_scatter_adamw's. */
+ * moments are updated: the kernel first forms postscale * *clip_coef in fp32, then g = (sum prescale * x) * that product.  At a
+ * coefficient of 1, and with a null one, the result is bit-identical to bg_reduce_scatter_adamw's.  Errors: bg_reduce_scatter_adamw's. */
 int bg_reduce_scatter_adamw_clipped(bg_ctx_t ctx, int gid, int lane, const size_t* src_offs, int src_dtype, float* param,
                                     float* exp_avg, float* exp_avg_sq, size_t shard_elems, float prescale, float postscale, float lr,
                                     float beta1, float beta2, float eps, float weight_decay, long long step, const float* clip_coef,
                                     void* stream);
 
 /* The same clipped AdamW rule on a local fp32 gradient `grad` of n elements (a multiple of 4): the step of units whose gradient
- * was reduced into an fp32 shard by the norm pass. */
+ * was reduced into an fp32 shard by the norm pass, with g = grad * *clip_coef (null: grad) rounded once.  Where the norm pass's
+ * postscale is a power of two, or the coefficient is 1, this step on its fp32 shard is bit-identical to
+ * bg_reduce_scatter_adamw_clipped on the same sources.  Errors, BG_EINVAL: those of bg_reduce_scatter_adamw, then n not a
+ * multiple of 4 or grad not 16-B aligned, then a null grad with n > 0. */
 int bg_adamw_clipped(float* param, float* exp_avg, float* exp_avg_sq, const float* grad, size_t n, float lr, float beta1,
                      float beta2, float eps, float weight_decay, long long step, const float* clip_coef, void* stream);
 

@@ -293,6 +293,96 @@ def test_collectives_reject_bad_arguments(bg):
     assert not bad, bad
 
 
+# Bad-argument calls of the optimizer entries (the AdamW reduce-scatter, its clipped form, the local clipped step and the norm
+# pass), with a null context.  Every hyperparameter is an exact fp32 value, so the message formats it as Python does.  Same child
+# process as above, with no device.
+_BAD_OPT_CALLS = r"""
+import ctypes, json, sys
+sys.path.insert(0, sys.argv[1])
+from hetu_galvatron_b200 import _bg
+L = _bg.lib()
+A, M = 0x10000, 0x10008            # a 16-B aligned and an 8-B aligned address; neither is ever dereferenced
+EINVAL = -1
+BF, F32 = 0, 1
+INF, NAN = float("inf"), float("nan")
+out = []
+def call(want_msg, name, *args):
+    before = L.bg_launch_count()
+    rc = getattr(L, name)(*args)
+    out.append(dict(call="%s%r" % (name, args), got=[rc, L.bg_last_error().decode(), L.bg_launch_count() - before],
+                    want=[EINVAL, want_msg, 0]))
+RSA, RSC, LOC, SSQ = "bg_reduce_scatter_adamw", "bg_reduce_scatter_adamw_clipped", "bg_adamw_clipped", "bg_reduce_scatter_sumsq"
+HYPER = dict(lr=1e-4, b1=0.5, b2=0.75, eps=1e-8, wd=0.0625, step=1)
+def rsa(p=A, m=A, v=A, **kw):
+    h = dict(HYPER, **kw)
+    return (None, 0, 1, None, BF, p, m, v, 64, 0.5, 0.25, h["lr"], h["b1"], h["b2"], h["eps"], h["wd"], h["step"], None)
+def rsc(p=A, m=A, v=A, **kw):
+    return rsa(p, m, v, **kw)[:-1] + (A, None)
+def loc(p=A, m=A, v=A, g=A, n=64, **kw):
+    h = dict(HYPER, **kw)
+    return (p, m, v, g, n, h["lr"], h["b1"], h["b2"], h["eps"], h["wd"], h["step"], A, None)
+STATE = "adamw: param, exp_avg and exp_avg_sq must be non-null"
+BAD = [(dict(lr=x), "adamw: lr %g must be finite and >= 0" % x) for x in (-1.0, INF, -INF, NAN)] + \
+      [(dict(eps=x), "adamw: eps %g must be finite and >= 0" % x) for x in (-0.5, INF, NAN)] + \
+      [(dict(wd=x), "adamw: weight_decay %g must be finite and >= 0" % x) for x in (-0.5, INF, NAN)] + \
+      [(dict(b1=x), "adamw: beta1 %g outside [0, 1)" % x) for x in (1.0, -0.5, 2.0, INF, NAN)] + \
+      [(dict(b2=x), "adamw: beta2 %g outside [0, 1)" % x) for x in (1.0, -0.5, 2.0, INF, NAN)] + \
+      [(dict(b1=0.99999999), "adamw: beta1 1 outside [0, 1)"),        # rounds to 1 in fp32
+       (dict(step=0), "adam step must be >= 1"), (dict(step=-(1 << 40)), "adam step must be >= 1")]
+for make in (rsa, rsc, loc):
+    name = {rsa: RSA, rsc: RSC, loc: LOC}[make]
+    for i in range(3):             # param, exp_avg, exp_avg_sq
+        p = [A] * 3; p[i] = None
+        call(STATE, name, *make(*p))
+        p = [A] * 3; p[i] = M
+        call("optimizer state not 16-B aligned", name, *make(*p))
+    for kw, msg in BAD:
+        call(msg, name, *make(**kw))
+    if make is loc:
+        call("adamw: 6 elements / gradient alignment (need multiples of 4, 16 B)", name, *make(n=6))
+        call("adamw: 64 elements / gradient alignment (need multiples of 4, 16 B)", name, *make(g=M))
+        call("adamw: null grad", name, *make(g=None))
+    else:                          # every hyperparameter edge that is valid, in turn: the context is checked next
+        for kw in (dict(lr=0.0, wd=0.0, b1=0.0, b2=0.0, eps=0.0), dict(b1=0.99999994, b2=0.99999994), dict(step=(1 << 31) + 5)):
+            call("null ctx", name, *make(**kw))
+def ssq(skip=(), dst=A, n=64, parts=A, n_parts=64):
+    flat = [x for r in skip for x in r]
+    arr = (ctypes.c_size_t * max(1, len(flat)))(*flat)
+    return (None, 0, 1, None, BF, dst, n, 0.5, 0.25, parts, n_parts, arr, len(skip), None)
+call("sum-of-squares partials missing", SSQ, *ssq(parts=None))
+call("sum-of-squares partials missing", SSQ, *ssq(n_parts=0))
+call("-1 skip ranges (at most 16)", SSQ, *ssq(skip=[(0, 8)] * 17)[:-2] + (-1, None))
+call("17 skip ranges (at most 16)", SSQ, *ssq(skip=[(0, 8)] * 17))
+for lo, hi in ((4, 8), (0, 12), (16, 8)):
+    call("skip range [%d, %d) is not 8-element aligned" % (lo, hi), SSQ, *ssq(skip=[(lo, hi)]))
+for lo, hi in ((0, 72), (64, 72), (72, 80)):
+    call("skip range [%d, %d) ends past the shard of 64 elements" % (lo, hi), SSQ, *ssq(skip=[(0, 8), (lo, hi)]))
+call("dst not 16-B aligned", SSQ, *ssq(dst=M))
+for skip in ([], [(0, 0)], [(0, 64)], [(56, 64), (0, 8), (0, 64)], [(8, 16)] * 16):
+    call("null ctx", SSQ, *ssq(skip=skip))
+call("null ctx", SSQ, *ssq(dst=None))
+print(json.dumps(out))
+"""
+
+
+def test_optimizer_rejects_bad_arguments(bg):
+    """The AdamW entries (the reduce-scatter, its clipped form and the local clipped step) reject, with BG_EINVAL and zero launches
+    and before they look at the context: a null or misaligned optimizer state, step < 1, lr, eps or weight_decay negative or not
+    finite, and beta1 or beta2 outside [0, 1) or NaN -- as fp32 values, so a beta that rounds to 1 is refused (beta1 = 1 would
+    turn every parameter into inf or NaN); the local step also a null gradient.  The norm pass rejects a skip range that ends
+    past the shard, as well as missing partials, too many ranges and misaligned or inverted ranges.  Valid edges (lr, wd, eps
+    and the betas 0; the largest fp32 beta below 1; a step past 2^31; empty, whole-shard, overlapping and BG_MAX_SKIP ranges)
+    pass every check and fail on the null context."""
+    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
+    res = subprocess.run([sys.executable, "-c", _BAD_OPT_CALLS, ROOT], env=env, capture_output=True, text=True, timeout=300)
+    assert res.returncode == 0, res.stderr
+    calls = json.loads(res.stdout.strip().splitlines()[-1])
+    n_bad = 4 + 3 + 3 + 5 + 5 + 3
+    assert len(calls) == 2 * (6 + n_bad + 3) + (6 + n_bad + 3) + (2 + 2 + 3 + 3 + 1 + 5 + 1)
+    bad = [c for c in calls if c["got"] != c["want"]]
+    assert not bad, bad
+
+
 def test_c_mirror_of_group_builder_matches_goldens(bg):
     L = bg.lib()
     gold = json.load(open(os.path.join(ROOT, "tests", "golden", "comm_groups.json")))
