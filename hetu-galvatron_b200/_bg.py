@@ -98,6 +98,8 @@ SIGNATURES = {
     "bg_bias_tanh": (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _vp]),
     "bg_swin_window_qkv_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
     "bg_swin_window_qkv_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
+    "bg_swin_rel_bias_fwd": (_i, [_vp, _i, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
+    "bg_swin_rel_bias_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),
     "bg_cross_attn_qkv_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _vp]),
     "bg_cross_attn_qkv_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _ll, _ll, _ll, _ll, _ll, _vp]),
     "bg_swin_window_merge_fwd": (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _ll, _ll, _ll, _ll, _vp]),

@@ -793,6 +793,33 @@ class CudaBackend:
                                                            heads, hn, _s()))
         return dmixed, dbp.sum(0)
 
+    def swin_rel_bias_fwd(self, table, index, shift_mask, mb, n_windows, window):
+        """table [(2w-1)^2, heads] (bf16 / fp32), index int32 [L * L], shift_mask uint8 [n_windows, L, L] or None -> the additive bf16
+        mask [mb * n_windows, heads, L, L]: a view of rows padded to a multiple of 8 columns, the stride the memory-efficient
+        attention kernel takes without a copy."""
+        L, heads = window * window, table.shape[1]
+        ld = (L + 7) // 8 * 8
+        out = torch.empty(mb * n_windows, heads, L, ld, dtype=torch.bfloat16, device=table.device)
+        self.bg.check(self.bg.lib().bg_swin_rel_bias_fwd(_p(table), self.bg.dtype_code(table.dtype), _p(index),
+                                                         _p(shift_mask) if shift_mask is not None else None, _p(out), mb, n_windows,
+                                                         heads, window, L, ld, _s()))
+        return out[..., :L]
+
+    def swin_rel_bias_bwd(self, dbias, cells, offsets, n_windows, window):
+        """dbias [mb * n_windows, heads, L, L] bf16 (rows may be padded) -> the table's gradient [(2w-1)^2, heads] fp32; cells / offsets
+        list the cells of every table entry (WindowLayout.rel_maps)."""
+        n, heads, L = dbias.shape[0], dbias.shape[1], dbias.shape[2]
+        ld = dbias.stride(2)
+        if dbias.stride(3) != 1 or ld % 8 or ld < L or dbias.stride(1) != L * ld or dbias.stride(0) != heads * L * ld:
+            ld = (L + 7) // 8 * 8
+            dbias = torch.nn.functional.pad(dbias, (0, ld - L))
+        n_table = (2 * window - 1) ** 2
+        npart = max(1, min(n, -(-self.norm_partials // heads)))
+        part = torch.empty(npart, n_table, heads, dtype=torch.float32, device=dbias.device)
+        self.bg.check(self.bg.lib().bg_swin_rel_bias_bwd(_p(dbias), _p(cells), _p(offsets), _p(part), npart, n // n_windows, n_windows,
+                                                         heads, window, L, ld, _s()))
+        return part.sum(0)
+
     # ---- T5 cross-attention: the query / key_value projections' outputs <-> the attention layout (include/bg_galvatron.h)
     def cross_attn_qkv_fwd(self, q_mixed, q_bias, kv_mixed, kv_bias, heads, hn):
         """q_mixed [s_q, b, heads * hn] + q_bias, kv_mixed [s_k, b, heads * 2 * hn] (per head k | v) + kv_bias -> q [b, s_q, heads, hn],
@@ -1003,21 +1030,27 @@ class CudaBackend:
         # the reference casts cos/sin to the activation dtype before applying them (apply_rotary_pos_emb)
         return torch.cos(freqs).to(dtype).float().contiguous(), torch.sin(freqs).to(dtype).float().contiguous()
 
-    def attention(self, q, k, v, causal, softmax_scale, key_mask=None, dropout_p=0.0, window_mask=None):
+    def attention(self, q, k, v, causal, softmax_scale, key_mask=None, dropout_p=0.0, window_mask=None, window_bias=None):
         """Attention is a LIBRARY call, as in the reference (transformer.py:495 calls flash-attn; K3 is not a collective and
         is outside the hot-path scope).  The default is cuDNN's fused SDPA, reached
         through torch SDPA; HGB_ATTN=flash selects flash-attn 2.  q [b,s,n,d], k/v [b,s,ng,d] (GQA un-expanded).  Differentiable.
         ``dropout_p`` > 0: dropout on the attention probabilities (transformer.py:443-503), drawn from torch's CUDA generator (the
         caller runs this under the model-parallel RNG tracker); SDPA may then pick the flash or memory-efficient kernel instead of
-        cuDNN's."""
+        cuDNN's.  ``window_mask`` / ``window_bias``: Swin's additive shift mask, or its learned relative-position bias (differentiable).
+        """
         import torch.nn.functional as F
         from torch.nn.attention import SDPBackend, sdpa_kernel
-        if window_mask is not None:
-            # Swin's shifted windows: an additive [windows, 1, L, L] mask (0 / -inf, q's dtype), one row of windows per sample
+        if window_mask is not None or window_bias is not None:
+            # Swin's shifted windows: an additive [windows, 1, L, L] mask (0 / -inf, q's dtype), one row of windows per sample; or
+            # the relative-position bias [windows, heads, L, L] (shift mask included), which needs its gradient: cuDNN's backward
+            # returns only dq, dk and dv, the memory-efficient kernel's also the bias gradient, so the bias pins that kernel (also
+            # where no gradient is taken, so that a checkpointed block's recompute runs the forward's kernel)
             assert not causal and key_mask is None and dropout_p == 0.0
-            with sdpa_kernel([SDPBackend.CUDNN_ATTENTION, SDPBackend.EFFICIENT_ATTENTION, SDPBackend.MATH]):
-                o = F.scaled_dot_product_attention(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), attn_mask=window_mask,
-                                                   scale=softmax_scale)
+            backends = [SDPBackend.EFFICIENT_ATTENTION] if window_bias is not None else \
+                [SDPBackend.CUDNN_ATTENTION, SDPBackend.EFFICIENT_ATTENTION, SDPBackend.MATH]
+            with sdpa_kernel(backends):
+                o = F.scaled_dot_product_attention(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2),
+                                                   attn_mask=window_bias if window_bias is not None else window_mask, scale=softmax_scale)
             return o.transpose(1, 2)
         if key_mask is not None:
             # BERT's padding mask (bert_hf/BertModel_sequential.py: get_extended_attention_mask): key j of sample b is visible iff

@@ -1910,6 +1910,149 @@ extern "C" int bg_drop_path_add_bwd(const void* dy, void* dx, float* dbias_parti
                                    iteration, site, stream);
 }
 
+// ---- Swin relative-position bias (HF SwinSelfAttention.relative_position_bias_table) ------------------------------------------
+// The additive attention mask of one block, [mb * nW][heads][L][ld] bf16 (ld >= L, a multiple of 8; columns L .. ld - 1 zero):
+// element (n, h, i, j) = table[index[i * L + j]][h] rounded to bf16, or -inf where the shift mask of window n % nW separates i and j.
+// A thread forms one 16-B vector (8 columns of row i of window w, head h) and stores it for every sample b (window b * nW + w),
+// so the index, table and mask reads are shared by the mb copies.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) swin_rel_bias_fwd_kernel(const T* __restrict__ table, const int* __restrict__ index,
+                                                                     const unsigned char* __restrict__ mask, uint4* __restrict__ out,
+                                                                     long long mb, long long nW, int heads, int L, int lv) {
+    const size_t tile = (size_t)nW * heads * L * lv, stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t v = (size_t)blockIdx.x * blockDim.x + threadIdx.x; v < tile; v += stride) {
+        const size_t row = v / lv;
+        const int jv = (int)(v - row * lv);
+        const size_t wh = row / L;
+        const int i = (int)(row - wh * L);
+        const long long w = (long long)(wh / heads);
+        const int h = (int)(wh - (size_t)w * heads);
+        const unsigned char* mrow = mask != nullptr ? mask + ((size_t)w * L + i) * L : nullptr;
+        float f[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            const int j = jv * 8 + e;
+            f[e] = 0.f;
+            if (j < L) {
+                f[e] = (float)__ldg(table + (size_t)__ldg(index + i * L + j) * heads + h);
+                if (mrow != nullptr && __ldg(mrow + j)) f[e] = -INFINITY;
+            }
+        }
+        const uint4 packed = pack8(f);
+        for (long long b = 0; b < mb; ++b) st16(out + (size_t)b * tile + v, packed);
+    }
+}
+
+// Its backward: dtable_partial[p][t][h] = the sum, over the cells c = i * L + j listed for entry t (cells[offsets[t]] ..
+// cells[offsets[t + 1] - 1], in that order), of the fp32 sum over windows n = p, p + n_partial, ... (ascending) of dbias[n][h][i][j].
+// grid = (heads, n_partial); a thread owns whole 8-column vectors of the L x ld tile, so every sum has one fixed order.  The
+// per-cell sums wait in shared memory [L * L] fp32 for the gather by table entry.
+__global__ void __launch_bounds__(kThreads) swin_rel_bias_bwd_kernel(const uint4* __restrict__ dbias, const int* __restrict__ cells,
+                                                                     const int* __restrict__ offsets, float* __restrict__ partial,
+                                                                     long long N, int L, int lv, int n_table) {
+    extern __shared__ float cell_sum[];
+    const int h = blockIdx.x, heads = gridDim.x, p = blockIdx.y, np = gridDim.y;
+    const int nvec = L * lv;
+    const size_t step = (size_t)np * heads * nvec;
+    for (int u = threadIdx.x; u < nvec; u += blockDim.x) {
+        float acc[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc[e] = 0.f;
+        const uint4* src = dbias + ((size_t)p * heads + h) * nvec + u;
+        long long n = p;
+        for (; n + 3LL * np < N; n += 4LL * np, src += 4 * step) {
+            uint4 g[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) g[k] = ld16_stream(src + k * step);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                float f[8];
+                unpack8(g[k], f);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) acc[e] = __fadd_rn(acc[e], f[e]);
+            }
+        }
+        for (; n < N; n += np, src += step) {
+            float f[8];
+            unpack8(ld16_stream(src), f);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) acc[e] = __fadd_rn(acc[e], f[e]);
+        }
+        const int i = u / lv, j0 = (u - i * lv) * 8;
+#pragma unroll
+        for (int e = 0; e < 8; ++e)
+            if (j0 + e < L) cell_sum[i * L + j0 + e] = acc[e];
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < n_table; t += blockDim.x) {
+        float s = 0.f;
+        for (int k = __ldg(offsets + t), end = __ldg(offsets + t + 1); k < end; ++k) s = __fadd_rn(s, cell_sum[__ldg(cells + k)]);
+        partial[((size_t)p * n_table + t) * heads + h] = s;
+    }
+}
+
+static const size_t kRelBiasMaxSmem = 200 * 1024;
+
+static int rel_bias_args(long long mb, long long n_windows, long long heads, long long window, long long window_tokens, long long ld,
+                         const char* who) {
+    if (mb < 1 || n_windows < 1 || heads < 1 || window < 1)
+        return fail(BG_EINVAL, "%s: mb %lld, windows %lld, heads %lld and window %lld must be >= 1", who, mb, n_windows, heads, window);
+    if (window_tokens != window * window)
+        return fail(BG_EINVAL, "%s: window_tokens %lld is not window %lld squared", who, window_tokens, window);
+    if (ld < window_tokens || ld % 8)
+        return fail(BG_EINVAL, "%s: row stride %lld must be a multiple of 8 >= window_tokens %lld", who, ld, window_tokens);
+    if (heads > 65535 || (size_t)window_tokens * window_tokens * sizeof(float) > kRelBiasMaxSmem ||
+        mb * n_windows * heads * window_tokens * ld > (1LL << 40))
+        return fail(BG_EUNSUPPORTED, "%s: %lld heads, a %lld-token window or %lld windows is too large", who, heads, window_tokens,
+                    mb * n_windows);
+    return BG_OK;
+}
+
+extern "C" int bg_swin_rel_bias_fwd(const void* table, int table_dtype, const int* index, const unsigned char* shift_mask, void* bias,
+                                    long long mb, long long n_windows, long long heads, long long window, long long window_tokens,
+                                    long long ld, void* stream) {
+    const char* who = "bg_swin_rel_bias_fwd";
+    int rc = rel_bias_args(mb, n_windows, heads, window, window_tokens, ld, who);
+    if (rc) return rc;
+    if (table_dtype != BG_BF16 && table_dtype != BG_F32) return fail(BG_EUNSUPPORTED, "%s: table dtype %d", who, table_dtype);
+    if (table == nullptr || index == nullptr || bias == nullptr || (uintptr_t)table % (table_dtype == BG_F32 ? 4 : 2) ||
+        (uintptr_t)index % 4 || !BG_ALIGNED16(bias))
+        return fail(BG_EINVAL, "%s: pointers must be non-null (shift_mask may be) and aligned", who);
+    const int L = (int)window_tokens, lv = (int)(ld / 8);
+    const int grid = local_grid((size_t)n_windows * heads * L * lv, kThreads);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (table_dtype == BG_F32)
+        swin_rel_bias_fwd_kernel<float><<<grid, kThreads, 0, st>>>((const float*)table, index, shift_mask, (uint4*)bias, mb, n_windows,
+                                                                   (int)heads, L, lv);
+    else
+        swin_rel_bias_fwd_kernel<__nv_bfloat16><<<grid, kThreads, 0, st>>>((const __nv_bfloat16*)table, index, shift_mask, (uint4*)bias,
+                                                                           mb, n_windows, (int)heads, L, lv);
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
+extern "C" int bg_swin_rel_bias_bwd(const void* dbias, const int* cells, const int* offsets, float* dtable_partial, int n_partial,
+                                    long long mb, long long n_windows, long long heads, long long window, long long window_tokens,
+                                    long long ld, void* stream) {
+    const char* who = "bg_swin_rel_bias_bwd";
+    int rc = rel_bias_args(mb, n_windows, heads, window, window_tokens, ld, who);
+    if (rc) return rc;
+    if (n_partial < 1 || n_partial > 65535) return fail(BG_EINVAL, "%s: n_partial %d must be in [1, 65535]", who, n_partial);
+    if (dbias == nullptr || cells == nullptr || offsets == nullptr || dtable_partial == nullptr || !BG_ALIGNED16(dbias) ||
+        (uintptr_t)cells % 4 || (uintptr_t)offsets % 4 || (uintptr_t)dtable_partial % 4)
+        return fail(BG_EINVAL, "%s: pointers must be non-null and aligned", who);
+    const int L = (int)window_tokens;
+    const size_t smem = (size_t)L * L * sizeof(float);
+    if (smem > 48 * 1024)          // above the default dynamic shared memory (w = 12: 81 KiB)
+        BG_CUDA(cudaFuncSetAttribute(swin_rel_bias_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRelBiasMaxSmem));
+    const dim3 grid((unsigned)heads, (unsigned)n_partial, 1);
+    swin_rel_bias_bwd_kernel<<<grid, kThreads, smem, (cudaStream_t)stream>>>((const uint4*)dbias, cells, offsets, dtable_partial,
+                                                                              mb * n_windows, L, (int)(ld / 8),
+                                                                              (int)((2 * window - 1) * (2 * window - 1)));
+    BG_CHECK_LAUNCH();
+    return BG_OK;
+}
+
 // ---- T5 cross-attention ---------------------------------------------------------------------------------------------------------
 static int cross_attn_args(long long s_q, long long s_k, long long batch, long long heads, long long head_dim, const char* who) {
     if (s_q < 1 || s_k < 1 || batch < 1 || heads < 1 || head_dim < 8 || head_dim % 8)
@@ -1983,7 +2126,8 @@ int bg_preload_ops() {
                              K((swin_merge_ln_bwd_kernel<1, false>)), K((swin_merge_ln_bwd_kernel<2, true>)),
                              K((swin_merge_ln_bwd_kernel<2, false>)), K((swin_merge_ln_bwd_kernel<kMergeVpt, true>)),
                              K((swin_merge_ln_bwd_kernel<kMergeVpt, false>)), K(swin_mean_pool_kernel<true>),
-                             K(swin_mean_pool_kernel<false>), K(cross_attn_qkv_fwd_kernel), K(cross_attn_qkv_bwd_kernel)};
+                             K(swin_mean_pool_kernel<false>), K(cross_attn_qkv_fwd_kernel), K(cross_attn_qkv_bwd_kernel),
+                             K(swin_rel_bias_fwd_kernel<float>), K(swin_rel_bias_fwd_kernel<__nv_bfloat16>), K(swin_rel_bias_bwd_kernel)};
 #undef K
     for (const void* k : kernels) {
         cudaFuncAttributes attr;

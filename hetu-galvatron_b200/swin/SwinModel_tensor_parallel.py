@@ -6,7 +6,9 @@ per-sample drop path on the attention branch; a patch-merging row between stages
 Windows are HF ``SwinLayer``'s: ``roll(-s, -s)`` then contiguous ws x ws windows, window w with window w's shift mask.  Shift,
 partition and token padding are one int32 token map per layer shape (``token_map``): the QKV relayout writes q, k, v straight into
 window order and the merge kernel writes the attention output back into token rows, so no activation is rolled, permuted or copied
-in torch.  There is no relative-position bias (the reference's attention has none).
+in torch.  There is no relative-position bias by default (the reference's attention has none); the ``relative_position_bias``
+spec key gives every block HF's learned table (``SwinAttention_tp``), turned into the attention's additive mask by
+``bg_swin_rel_bias_fwd`` and its gradient folded back into the table by ``bg_swin_rel_bias_bwd``.
 
 Token padding: stage k runs ``config.tokens_run[k]`` tokens, the real ones followed by rows no kernel reads as input (the window
 relayout, the patch merge and the mean-pool address real tokens only), so their gradient is exactly zero
@@ -55,11 +57,20 @@ def shift_mask(res, window, shift):
     return label[:, :, None] != label[:, None, :]
 
 
+def relative_position_index(window):
+    """int64 [L * L]: HF ``SwinSelfAttention.create_relative_position_index`` flattened -- entry i * L + j is the table row of query
+    i and key j, (dy + w - 1) * (2w - 1) + dx + w - 1 for their offset (dy, dx) in the window."""
+    c = torch.stack(torch.meshgrid(torch.arange(window), torch.arange(window), indexing="ij")).flatten(1)
+    rel = c[:, :, None] - c[:, None, :] + (window - 1)
+    return (rel[0] * (2 * window - 1) + rel[1]).reshape(-1)
+
+
 class WindowLayout:
     """The token map of one (resolution, window, shift), its inverse and the additive shift mask, on each device once; the mask is
     expanded to mb * nW windows and cached per (mb, device, dtype), as ``_KeyMask`` caches.  One instance per layer shape, shared by
     every block of that shape (``window_layout``).  The expanded mask is materialised: its window axis is b * nW + w, which no
-    broadcast view of the [nW, L, L] mask expresses."""
+    broadcast view of the [nW, L, L] mask expresses.  With the relative-position bias, ``rel_maps`` holds what its kernels read:
+    the index, the shift mask as bytes, and the index's cells grouped by table entry (cells, offsets)."""
 
     def __init__(self, res, window, shift):
         self.res, self.window, self.shift = res, window, shift
@@ -68,13 +79,27 @@ class WindowLayout:
         m = token_map(res, window, shift)
         self._map, self._inv = m.to(torch.int32), torch.argsort(m).to(torch.int32)
         self._mask = shift_mask(res, window, shift)
-        self._dev, self._masks = {}, {}
+        self._dev, self._masks, self._rel = {}, {}, {}
 
     def maps(self, device):
         key = str(device)
         if key not in self._dev:
             self._dev[key] = (self._map.to(device), self._inv.to(device))
         return self._dev[key]
+
+    def rel_maps(self, device):
+        """(index int32 [L * L], shift mask uint8 [nW, L, L] or None, cells int32 [L * L] = the stable argsort of the index,
+        offsets int32 [(2w-1)^2 + 1]: entry t's cells are cells[offsets[t]:offsets[t + 1]], ascending) on ``device``."""
+        key = str(device)
+        if key not in self._rel:
+            index = relative_position_index(self.window)
+            counts = torch.bincount(index, minlength=(2 * self.window - 1) ** 2)
+            offsets = torch.cat([torch.zeros(1, dtype=torch.int64), counts.cumsum(0)])
+            cells = torch.argsort(index, stable=True)
+            mask = self._mask.to(torch.uint8) if self._mask is not None else None
+            self._rel[key] = tuple(t.to(device) if t is not None else None for t in
+                                   (index.to(torch.int32), mask, cells.to(torch.int32), offsets.to(torch.int32)))
+        return self._rel[key]
 
     def attn_mask(self, mb, device, dtype):
         if self._mask is None:
@@ -119,6 +144,23 @@ class _WindowMergeFn(torch.autograd.Function):
         layout, mb, heads, hn = ctx.dims
         tmap, inv = layout.maps(drows.device)
         return get_backend().swin_window_merge_bwd(drows, tmap, inv, layout.n_windows, mb, heads, hn), None, None, None
+
+
+class _RelBiasFn(torch.autograd.Function):
+    """The block's relative-position table -> its additive attention mask [mb * nW, heads, L, L] (bias + shift mask), and the
+    mask's gradient -> the table's."""
+
+    @staticmethod
+    def forward(ctx, table, layout, mb):
+        index, mask, _, _ = layout.rel_maps(table.device)
+        ctx.dims = (layout, table.dtype)
+        return get_backend().swin_rel_bias_fwd(table, index, mask, mb, layout.n_windows, layout.window)
+
+    @staticmethod
+    def backward(ctx, dbias):
+        layout, dt = ctx.dims
+        _, _, cells, offsets = layout.rel_maps(dbias.device)
+        return get_backend().swin_rel_bias_bwd(dbias, cells, offsets, layout.n_windows, layout.window).to(dt), None, None
 
 
 class _MergeLnFn(torch.autograd.Function):
@@ -166,9 +208,13 @@ def stage_config(mconf, stage):
 
 class SwinAttention_tp(nn.Module):
     """QKV (column-parallel, bias added by the window relayout) -> window attention -> merge to token rows -> projection
-    (row-parallel; + residual in its epilogue, or the drop path kernel)."""
+    (row-parallel; + residual in its epilogue, or the drop path kernel).
 
-    def __init__(self, mconf, tp_group):
+    With ``window`` (the relative-position bias): HF's ``relative_position_bias_table`` [(2w-1)^2, heads], split by heads over the
+    tensor-parallel group as the QKV projection is.  Its init is the original Swin's, truncated normal with std 0.02, drawn for the
+    whole table from a generator seeded by (seed, layer) so that every tensor-parallel layout holds slices of one table."""
+
+    def __init__(self, mconf, tp_group, window=None, layer_number=0):
         super().__init__()
         t = _size(tp_group)
         heads, c = mconf.num_attention_heads, mconf.hidden_size
@@ -180,6 +226,23 @@ class SwinAttention_tp(nn.Module):
         self.dense = RowParallelLinear(c, c, config=mconf, bias=True, skip_bias_add=True, input_is_parallel=True, tp_group=tp_group,
                                        device="meta")
         self.scale = self.hn ** -0.5
+        self.tp_group, self.layer_number = tp_group, layer_number
+        if window is not None:
+            self.relative_position_bias_table = nn.Parameter(torch.empty((2 * window - 1) ** 2, self.heads_local, device="meta"))
+        else:
+            self.relative_position_bias_table = None
+
+    def reset_parameters(self):
+        table = self.relative_position_bias_table
+        if table is None:
+            return
+        heads = table.shape[1] * _size(self.tp_group)
+        g = torch.Generator().manual_seed(get_args().seed * 1000003 + self.layer_number)
+        full = nn.init.trunc_normal_(torch.empty(table.shape[0], heads), std=0.02, generator=g)
+        r = self.tp_group.rank_in_group() if _size(self.tp_group) > 1 else 0
+        with torch.no_grad():
+            table.copy_(full[:, r * table.shape[1]:(r + 1) * table.shape[1]])
+        mark_tensor_parallel(table)
 
 
 class SwinBlock_tp(nn.Module):
@@ -190,7 +253,8 @@ class SwinBlock_tp(nn.Module):
         self.tp_group = tp_group.group if tp_group is not None else None
         c = stage["width"]
         self.layernorm_before = LayerNorm(c, eps=config.layer_norm_eps, device="meta")
-        self.attention = SwinAttention_tp(mconf, self.tp_group)
+        self.attention = SwinAttention_tp(mconf, self.tp_group, stage["window"] if config.relative_position_bias else None,
+                                          layer_number)
         self.layernorm_after = LayerNorm(c, eps=config.layer_norm_eps, device="meta")
         self.mlp = ParallelMLP(mconf, tp_group=self.tp_group, device="meta")
         self.layout = window_layout(stage["res"], stage["window"], stage["shift"] if shifted else 0)
@@ -203,11 +267,15 @@ class SwinBlock_tp(nn.Module):
         residual = hidden_states
         mixed, qkv_bias = a.query_key_value(self.layernorm_before(hidden_states))              # [t_run, mb, 3 C / t]
         q, k, v = _WindowQkvFn.apply(mixed, qkv_bias, self.layout, a.heads_local, a.hn)       # [mb * nW, L, heads / t, hn]
-        mask = self.layout.attn_mask(mb, q.device, q.dtype)
-        if mask is None:
-            ctxt = _attention(q, k, v, False, a.scale)
+        if a.relative_position_bias_table is not None:
+            bias = _RelBiasFn.apply(a.relative_position_bias_table, self.layout, mb)    # [mb * nW, heads / t, L, L]
+            ctxt = get_backend().attention(q, k, v, False, a.scale, window_bias=bias)
         else:
-            ctxt = get_backend().attention(q, k, v, False, a.scale, window_mask=mask)
+            mask = self.layout.attn_mask(mb, q.device, q.dtype)
+            if mask is None:
+                ctxt = _attention(q, k, v, False, a.scale)
+            else:
+                ctxt = get_backend().attention(q, k, v, False, a.scale, window_mask=mask)
         ctxt = _WindowMergeFn.apply(ctxt, self.layout, mb, hidden_states.shape[0])            # [t_run, mb, C / t]
         if self.drop_path > 0.0 and self.training:
             batch = dropout_random.get_context().batch

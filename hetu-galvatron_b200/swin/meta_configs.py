@@ -1,9 +1,11 @@
 """Swin model shapes (``galvatron/models/swin/meta_configs/swin-*.json`` + ``config_utils.py``).  ``config_from_meta`` takes a
-shipped name or a dict spec {embed_dim, depths, num_heads, window_size, image_size, patch_size, ...}."""
+shipped name or a dict spec {embed_dim, depths, num_heads, window_size, image_size, patch_size, ...}.  ``relative_position_bias``
+(False in both shipped specs, the reference's model) gives every block HF's learned relative-position table."""
 import types
 
 _COMMON = dict(patch_size=4, num_channels=3, num_labels=1000, layer_norm_eps=1e-5, mlp_ratio=4, drop_path_rate=0.1,
-               hidden_dropout_prob=0.0, attention_probs_dropout_prob=0.0, use_absolute_embeddings=False)
+               hidden_dropout_prob=0.0, attention_probs_dropout_prob=0.0, use_absolute_embeddings=False,
+               relative_position_bias=False)
 _SPECS = {
     "swin-huge-patch4-window7-224": dict(_COMMON, embed_dim=320, depths=[2, 2, 42, 2], num_heads=[8, 16, 32, 64], window_size=7,
                                          image_size=224),
@@ -38,7 +40,8 @@ def config_from_meta(model_type):
         image_size=p["image_size"], patch_size=p["patch_size"], num_channels=p["num_channels"], num_labels=p["num_labels"],
         layer_norm_eps=p["layer_norm_eps"], mlp_ratio=p["mlp_ratio"], drop_path_rate=float(p["drop_path_rate"]),
         hidden_dropout_prob=float(p["hidden_dropout_prob"]), attention_probs_dropout_prob=float(p["attention_probs_dropout_prob"]),
-        use_absolute_embeddings=bool(p["use_absolute_embeddings"]), hidden_act="gelu_pytorch_tanh",
+        use_absolute_embeddings=bool(p["use_absolute_embeddings"]), relative_position_bias=bool(p["relative_position_bias"]),
+        hidden_act="gelu_pytorch_tanh",
         model_name=model_type if isinstance(model_type, str) else "custom")
     config.num_hidden_layers = sum(config.depths)
     config.stages = stage_geometry(config)

@@ -342,6 +342,22 @@ int bg_swin_window_qkv_fwd(const void* mixed, const void* bias, const int* map, 
 int bg_swin_window_qkv_bwd(const void* dq, const void* dk, const void* dv, void* dmixed, float* dbias_partial, int n_partial,
                            const int* inv, long long mb, long long tokens, long long tokens_run, long long n_windows,
                            long long window_tokens, long long heads, long long head_dim, void* stream);
+/* Swin's learned relative-position bias (HF SwinSelfAttention.relative_position_bias_table), window w, L = window_tokens = w * w,
+ * (2w-1)^2 table entries.  bg_swin_rel_bias_fwd: table [(2w-1)^2][heads] (table_dtype BG_BF16 or BG_F32), index int32 [L * L]
+ * (HF's relative_position_index, entries < (2w-1)^2) and shift_mask uint8 [n_windows][L][L] (non-zero where HF's shift mask separates
+ * query i and key j; NULL when the block is not shifted) -> bias [mb * n_windows][heads][L][ld] bf16, window b * n_windows + w of
+ * sample b: element (n, h, i, j) = table[index[i * L + j]][h] rounded to bf16, or -inf where shift_mask[n % n_windows][i][j] != 0;
+ * columns L .. ld - 1 zero.  bg_swin_rel_bias_bwd: the gradient of that bias, same layout, -> dtable_partial [n_partial][(2w-1)^2]
+ * [heads] fp32: partial p sums windows p, p + n_partial, ... and, for entry t, the cells c = i * L + j in the order cells[offsets[t]]
+ * .. cells[offsets[t + 1] - 1] (the caller lists every cell with index t there, once); the caller adds the rows.  The order of every
+ * sum is fixed, so the result is deterministic.  The index, cells and offsets are not checked.  BG_EINVAL for a size < 1,
+ * window_tokens != window^2, ld not a multiple of 8 >= window_tokens, n_partial outside [1, 65535] and null or misaligned pointers
+ * (bias / dbias 16-B, table its element size, the int32 arrays and dtable_partial 4-B); BG_EUNSUPPORTED for a table dtype other than
+ * BG_BF16 / BG_F32, more than 65535 heads or a window above 15 x 15 tokens per side (L * L fp32 > 200 KiB of shared memory). */
+int bg_swin_rel_bias_fwd(const void* table, int table_dtype, const int* index, const unsigned char* shift_mask, void* bias, long long mb,
+                         long long n_windows, long long heads, long long window, long long window_tokens, long long ld, void* stream);
+int bg_swin_rel_bias_bwd(const void* dbias, const int* cells, const int* offsets, float* dtable_partial, int n_partial, long long mb,
+                         long long n_windows, long long heads, long long window, long long window_tokens, long long ld, void* stream);
 /* T5 cross-attention (t5/T5Model_tensor_parallel.py): the two projections' outputs -> the attention library's layout.
  * bg_cross_attn_qkv_fwd: q_mixed [s_q * batch][heads * head_dim] + q_bias and kv_mixed [s_k * batch][heads * 2 * head_dim] (per head
  * k | v) + kv_bias, SBH rows (row = token * batch + sample) -> q [batch][s_q][heads][head_dim], k, v [batch][s_k][heads][head_dim];

@@ -1,6 +1,7 @@
 """Swin on one GPU: training steps of Swin-H/224 through the public API, and the Swin kernels alone next to the eager torch sequence
 each replaces (CUDA events, warm-up).
-Usage: python scripts/bench_swin.py [--steps N] [--warmup W] [--batch B] [--skip-steps]  -> JSON lines on stdout.
+Usage: python scripts/bench_swin.py [--steps N] [--warmup W] [--batch B] [--skip-steps] [--relative-position-bias]
+  -> JSON lines on stdout.
 
   * "card": the GPU's name, power limit and maximum SM clock, read in the same run as the numbers.
   * "kernel": each Swin kernel at Swin-H/224 shapes (micro-batch B): time per call and achieved bytes/s, the bytes being what the
@@ -9,7 +10,10 @@ Usage: python scripts/bench_swin.py [--steps N] [--warmup W] [--batch B] [--skip
   * "attention": the window-attention library calls of one step (forward + backward of every block at its stage's shape), timed
     alone, and their share of the step.
   * "step": s/step, images/s, torch peak memory and the peer-memory arena at batch B (no padding tokens when 196 B and 49 B are
-    multiples of 8) and at batch B - 1 (stages 2 and 3 then run 200 and 56 tokens), each measured in a process of its own."""
+    multiples of 8) and at batch B - 1 (stages 2 and 3 then run 200 and 56 tokens), each measured in a process of its own.
+  * --relative-position-bias: also the two bias kernels at every stage's shape (bytes: the bf16 mask written / its gradient read),
+    the window attention of one step with the bias ("attention_bias": the memory-efficient kernel, the bias gradient included)
+    next to the plain one, and the step at batch B without and with the bias, alternated twice."""
 import argparse
 import json
 import os
@@ -55,13 +59,13 @@ def _emit(name, stage, ms, nbytes, eager_ms=None):
     print(json.dumps(rec), flush=True)
 
 
-def kernels(batch):
+def kernels(batch, rel_bias=False):
     from hetu_galvatron_b200.core.runtime.backend import CudaBackend
     from hetu_galvatron_b200.swin import config_from_meta
     from hetu_galvatron_b200.swin.SwinModel_tensor_parallel import WindowLayout
     be = CudaBackend(arena_bytes=64 << 20)
     config = config_from_meta(SPEC)
-    attn_ms = 0.0
+    attn_ms = attn_bias_ms = 0.0
     for k, st in enumerate(config.stages):
         res, c, heads, ws = st["res"], st["width"], st["heads"], st["window"]
         hn, t = c // heads, st["tokens"]
@@ -99,6 +103,19 @@ def kernels(batch):
                 be.attention(qg, kg, vg, False, hn ** -0.5)
             o.backward(torch.ones_like(o))
         attn_ms += st["depth"] * timeit(attn, iters=10, warm=2)
+        if rel_bias:
+            index, smask, cells, offsets = lay.rel_maps("cuda")
+            table = (0.02 * torch.randn((2 * ws - 1) ** 2, heads, device="cuda")).to(BF)
+            rb = be.swin_rel_bias_fwd(table, index, smask, batch, lay.n_windows, ws)
+            nbytes = rb.numel() // (ws * ws) * ((ws * ws + 7) // 8 * 8) * 2
+            _emit("swin_rel_bias_fwd", k, timeit(lambda: be.swin_rel_bias_fwd(table, index, smask, batch, lay.n_windows, ws)), nbytes)
+            _emit("swin_rel_bias_bwd", k, timeit(lambda: be.swin_rel_bias_bwd(rb, cells, offsets, lay.n_windows, ws)), nbytes)
+            rbg = rb.detach().requires_grad_(True)
+
+            def attn_bias():
+                o = be.attention(qg, kg, vg, False, hn ** -0.5, window_bias=rbg)
+                o.backward(torch.ones_like(o))
+            attn_bias_ms += st["depth"] * timeit(attn_bias, iters=10, warm=2)
         if k + 1 < len(config.stages):
             w4, b4 = torch.ones(4 * c, device="cuda").to(BF), torch.zeros(4 * c, device="cuda").to(BF)
             to = t // 4
@@ -128,10 +145,10 @@ def kernels(batch):
             dy = torch.randn(rows, c, device="cuda").to(BF)
             _emit("swin_mean_pool_bwd", k, timeit(lambda: be.swin_mean_pool_bwd(dy, t, t, batch)), act + rows * c * 2)
     be.close()
-    return attn_ms
+    return attn_ms, attn_bias_ms
 
 
-def steps(batch, n_steps, warmup):
+def steps(batch, n_steps, warmup, rel_bias=False):
     import smoke_model as sm
     from hetu_galvatron_b200.core.runtime.backend import reset_backend
     from hetu_galvatron_b200.core.runtime.utils import get_optimizer_and_param_scheduler
@@ -139,6 +156,7 @@ def steps(batch, n_steps, warmup):
     reset_backend()
     args = sm.tiny_args(global_train_batch_size=batch, chunks=1, default_dp_type="zero2", init_method_std=0.02, lr=1e-4)
     config = set_model_config(config_from_meta(SPEC), args)
+    config.relative_position_bias = rel_bias
     model = swin_model_hp(config, args)
     opt, _ = get_optimizer_and_param_scheduler(model, args)
     g = torch.Generator(device="cuda").manual_seed(0)
@@ -161,7 +179,7 @@ def steps(batch, n_steps, warmup):
     e.record()
     torch.cuda.synchronize()
     sec = s.elapsed_time(e) / 1e3 / n_steps
-    rec = dict(step="swin-h/224", batch=batch, tokens_run=config.tokens_run, s_per_step=round(sec, 4), images_per_s=round(batch / sec, 1),
+    rec = dict(step="swin-h/224", relative_position_bias=rel_bias, batch=batch, tokens_run=config.tokens_run, s_per_step=round(sec, 4), images_per_s=round(batch / sec, 1),
                first_loss=round(losses[0], 4), last_loss=round(losses[-1], 4),
                torch_peak_GiB=round(torch.cuda.max_memory_allocated() / 2**30, 1), arena_GiB=round(args.arena_bytes / 2**30, 2))
     print(json.dumps(rec), flush=True)
@@ -172,10 +190,11 @@ def steps(batch, n_steps, warmup):
     return sec
 
 
-def _steps_in_child(batch, n_steps, warmup):
+def _steps_in_child(batch, n_steps, warmup, rel_bias=False):
     """one step measurement in a process of its own, so that nothing the previous model allocated or cached counts in its memory"""
     out = subprocess.run([sys.executable, os.path.abspath(__file__), "--only-steps", "--batch", str(batch), "--steps", str(n_steps),
-                          "--warmup", str(warmup)], capture_output=True, text=True, check=True).stdout
+                          "--warmup", str(warmup)] + (["--relative-position-bias"] if rel_bias else []), capture_output=True, text=True,
+                         check=True).stdout
     rec = json.loads([ln for ln in out.splitlines() if ln.startswith("{")][-1])
     print(json.dumps(rec), flush=True)
     return rec["s_per_step"]
@@ -187,20 +206,28 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--skip-steps", action="store_true")
+    ap.add_argument("--relative-position-bias", action="store_true", help="also measure the model with HF's relative-position bias")
     ap.add_argument("--only-steps", action="store_true", help="(internal) one step measurement at --batch in this process")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_swin.py measures on a GPU"
     if a.only_steps:
-        steps(a.batch, a.steps, a.warmup)
+        steps(a.batch, a.steps, a.warmup, a.relative_position_bias)
         return
     card()
-    attn_ms = kernels(a.batch)
+    attn_ms, attn_bias_ms = kernels(a.batch, a.relative_position_bias)
     torch.cuda.empty_cache()
     if a.skip_steps:
         return
     sec = _steps_in_child(a.batch, a.steps, a.warmup)
     print(json.dumps(dict(attention="window attention fwd + bwd of every block, timed alone", batch=a.batch, ms=round(attn_ms, 2),
                           share_of_step=round(attn_ms / (sec * 1e3), 4))), flush=True)
+    if a.relative_position_bias:
+        sec_bias = _steps_in_child(a.batch, a.steps, a.warmup, True)
+        print(json.dumps(dict(attention_bias="window attention fwd + bwd of every block with the relative-position bias (memory-"
+                              "efficient kernel), timed alone", batch=a.batch, ms=round(attn_bias_ms, 2),
+                              share_of_step=round(attn_bias_ms / (sec_bias * 1e3), 4))), flush=True)
+        _steps_in_child(a.batch, a.steps, a.warmup)
+        _steps_in_child(a.batch, a.steps, a.warmup, True)
     _steps_in_child(a.batch - 1, a.steps, a.warmup)
 
 
